@@ -4,11 +4,11 @@
 //
 // It is the gather half of the two split forms of chebyshev5 (lib/models.py:69-103) the host uses next to the fused
 // kernel:
-//   contract first:  Z = X . [W_0 | W_1 | ... ] on the TMA-fed tensor-core kernel (gemm_tc.cu), then
+//   contract first:  Z = X . [W_0 | W_1 | ... ] on the tensor-core kernel (ellconv_tc.cu), then
 //                    out = epi( sum_k op_k Z_k )                 -- the operators touch Fout-wide rows instead of Fin-wide
 //                    ones, and the contraction runs over the (fewer) rows of the coarse level when op_k un-pools;
 //   basis first:     B_k = op_k X (this kernel, written where the weight gradient wants it anyway), then the
-//                    contraction of plain tensors on the TMA-fed kernel.
+//                    contraction of plain tensors on the tensor-core kernel.
 // A pure SIMT kernel: one float4 column group of one row per thread, two rows in flight per thread (eight independent
 // neighbour-row loads), no shared-memory tiles -- so all 64 warps of an SM are resident, the L1 is ~200 KB and a CTA's
 // 64 consecutive rows re-hit each other's one-rings in it.  Bound: L2 -> SM bandwidth of the neighbour rows.
@@ -20,7 +20,7 @@ namespace cape {
 namespace {
 
 constexpr int AP_THREADS = 256;
-constexpr int AP_ROWS = 128;           // rows per CTA (measured: 64 -> 128 = -0.06 ms/step; experiment knob 10 overrides)
+constexpr int AP_ROWS = 128;           // rows per CTA (experiment knob 10 overrides)
 constexpr int AP_QS = 3072;            // floats of condition vectors per CTA
 
 struct ApTerm {

@@ -8,6 +8,9 @@
 
 namespace cape {
 
+// SM count of the H100 SXM: grid caps of the grid-stride kernels are small multiples of it
+constexpr int H100_SMS = 132;
+
 void set_error(const std::string& msg);
 void count_launches(int n);   // bookkeeping for cape_launch_count()
 
@@ -39,7 +42,7 @@ struct EllOp {
 
 struct cape_topology {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = cape::H100_SMS;   // replaced by the device's count when the handle is created
   std::vector<cape::EllOp> ops;
   void* workspace = nullptr;
   int64_t workspace_bytes = 0;

@@ -711,8 +711,6 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
   if (a->epilogue == CAPE_EPI_AFFINE) CAPE_REQUIRE(dual, "AFFINE epilogue needs a w2 term");
   if (a->epilogue == CAPE_EPI_SLOPE || a->epilogue == CAPE_EPI_DUALMASK) CAPE_REQUIRE(a->aux, "epilogue needs aux");
   p.wvec = wvec ? 1 : 0;
-  p.split_rn = g_tuning[0];
-  p.precise = a->precise;
   p.ovec = (a->ncols % 4 == 0) && aligned16(a->out) && (!a->out2 || aligned16(a->out2)) && (!a->aux || aligned16(a->aux));
   const int BNsel = a->ncols <= 32 ? 32 : 64;
   if (p.nslots > 0) {
@@ -723,17 +721,17 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
   if (a->plain_only) {
     const int rc = launch_gemm_tc(t, p, dual, st);
     if (rc != 0) return rc < 0 ? rc : 0;
-    CAPE_REQUIRE(false, "plain_only call not eligible for the TMA-fed kernel (needs the tensor-core path, all terms "
-                        "identity with wT and wT_lo, ncols % 16 == 0, 16-byte aligned operands)");
+    CAPE_REQUIRE(false, "plain_only call not eligible for the tensor-core contraction (needs the tensor-core path, all "
+                        "terms identity with wT, ncols % 16 == 0, 16-byte aligned operands)");
   }
   {
     int rc = launch_thin_fwd(t, p, dual, st);             // <= 4 input channels: streaming kernel
     if (rc != 0) return rc < 0 ? rc : 0;
     rc = launch_thinout_fwd(t, p, dual, st);              // <= 4 output columns: contract first, then gather
     if (rc != 0) return rc < 0 ? rc : 0;
-    rc = launch_gemm_tc(t, p, dual, st);                  // plain operands only: TMA-fed tcgen05 contraction
+    rc = launch_gemm_tc(t, p, dual, st);                  // plain operands only: wgmma contraction
     if (rc != 0) return rc < 0 ? rc : 0;
-    rc = launch_ellconv_tc(t, p, dual, st);               // tcgen05 path when eligible (writes the stashes itself)
+    rc = launch_ellconv_tc(t, p, dual, st);               // wgmma path when eligible (writes the stashes itself)
     if (rc != 0) return rc < 0 ? rc : 0;
   }
   if (any_stash) {                                        // fp32-pipe path: the basis copies come from the resample kernel
@@ -810,9 +808,7 @@ static int dw_single(cape_topology* t, const cape_dw_args* a, void* stream) {
     int rc = launch_thin_dw(t, a, &p.op, 1, &ns, (cudaStream_t)stream);           // <= 4 input channels
     if (rc < 0) return rc;
     if (rc == 1) always_reduce = true;                                            // partials always in the workspace
-    else rc = launch_dw_dense_tma(t, a, p.op, &ns, (cudaStream_t)stream);         // dense operands: TMA + tcgen05
-    if (rc < 0) return rc;
-    if (rc == 0) rc = launch_ellconv_dw_tc(t, a, p.op, &ns, (cudaStream_t)stream);   // gathered basis: tcgen05
+    else rc = launch_ellconv_dw_tc(t, a, p.op, &ns, (cudaStream_t)stream);        // tensor cores (wgmma)
     if (rc < 0) return rc;
     if (rc == 1) {
       if (ns > 1 || always_reduce) {

@@ -1,13 +1,13 @@
-// tcgen05 weight-gradient kernel:  dW_t[f, c] = sum_{n,v} A_t[n,v,f] * G[n,v,c]   (3xTF32, fp32 accumulate in TMEM)
+// Tensor-core (wgmma, sm_90a) weight-gradient kernel:  dW[f, c] = sum_{n,v} A[n,v,f] * G[n,v,c]   (3xTF32, fp32
+// accumulation), for gathered basis operands (A = op . X) and plain ones (A = X) alike.
 //
-// The reduction runs over the rows (up to N*6890 = 441k), so rows are the MMA K dimension and both operands are
-// "MN-major": the gathered basis rows A[row, f0..f0+127] (M = f contiguous) and the upstream-gradient rows
-// G[row, c..] (N = c contiguous) are written to shared memory exactly as they are read from HBM -- 128-byte
-// row segments -- in the one MN-major layout tcgen05 accepts for 32-bit operands, SWIZZLE_128B_BASE32B
-// (cute Layout_MN_SW128_32B_Atom: 4 k-rows x 32 floats per 512-byte atom, 32-byte chunks XOR-ed with the k-row).
-// One CTA owns a 128-wide slice of f, ALL output columns (<= 512 TMEM columns) and one split of the rows; the
-// basis chunk is gathered once per 32 rows and reused by every 128-column sub-tile of G.  Partial sums of the row
-// splits go to the topology workspace and are reduced deterministically (reduce_splits_kernel).
+// The reduction runs over the rows (up to N*6890), so rows are the MMA K dimension.  wgmma reads 32-bit operands
+// K-major only, so the producers transpose on the way into shared memory: lane k of a warp loads row k of the chunk
+// (a float4 of four consecutive f, or c for G) and writes the four values into four tile rows at column k -- in the
+// swizzled layout the 32 lanes of one such store hit 32 different banks.  One CTA (two warpgroups, 64 f each) owns a
+// 128-wide slice of f, a BN-wide slice of the output columns and one split of the rows; the chunks are
+// double-buffered as in ellconv_tc.cu.  Partial sums of the row splits go to the topology workspace and are reduced
+// deterministically (reduce_splits_kernel).
 #include "common.cuh"
 #include "ellconv_params.cuh"
 #include "tc_common.cuh"
@@ -16,20 +16,11 @@ namespace cape {
 
 namespace {
 
-constexpr int DT_PROD_WARPS = 8;
-constexpr int DT_PROD_THREADS = DT_PROD_WARPS * 32;
-constexpr int DT_THREADS = DT_PROD_THREADS + 32;
-constexpr int DT_KCH = 32;                         // rows (K) per pipeline stage = 4 MMAs of K=8
-constexpr int DT_A_TILE = 4 * 4096;                // 128 f x 32 rows, hi or lo
-constexpr int DT_MAX_STAGES = 4;
-using namespace tc;     // mbarriers, fences, UMMA issue, TMEM loads, MN-major descriptors (tc_common.cuh)
+using namespace tc;
 
-// byte offset of the 16-byte chunk `ch` (0..7) of MN block `mb`, k-row `row` (0..31) inside an operand tile:
-// block stride 4096, 4-row group stride 512, row stride 128, 32-byte chunk index XOR (row & 3)  [Swizzle<2,5,2>]
-__device__ __forceinline__ uint32_t mn_off(int mb, int row, int ch) {
-  const int kr = row & 3;
-  return (uint32_t)(mb * 4096 + (row >> 2) * 512 + kr * 128 + ((((ch >> 1) ^ kr) << 5) | ((ch & 1) << 4)));
-}
+constexpr int DW_THREADS = 256;
+constexpr int DW_KCH = 32;                   // rows (K) per chunk
+constexpr int DW_A_TILE = 128 * 128;         // 128 f x 32 rows, hi or lo
 
 struct DwTcParams {
   int rows_out, ncols, F, src_rows, src_stride;
@@ -39,231 +30,141 @@ struct DwTcParams {
   const float* g;
   float* out;          // dw (nsplit == 1) or workspace [nsplit, F, ncols]
   long long out_rs;
-  int nsplit, accumulate, ovec;
+  int nsplit, accumulate;
 };
 
-// OCC = CTAs per SM the configuration is sized for: narrow outputs (ncols <= 128) run two CTAs per SM (twice the warps
-// to hide the load latency; 2 x ~97 KB shared memory, <= 112 registers, <= 256 TMEM columns each); wide outputs
-// (ncols >= 256) need the TMEM and deeper rings of a single CTA (measured: 1.7x slower with two).
-template <int BN, int OCC>
-struct DtCfg {
-  static constexpr int G_TILE = (BN / 32) * 4096;             // BN columns x 32 rows, hi or lo
-  static constexpr int A_STAGE = 2 * DT_A_TILE;
-  static constexpr int G_STAGE = 2 * G_TILE;
-  static constexpr int A_STAGES = OCC == 2 ? 2 : 3;
-  static constexpr int G_STAGES = OCC == 2 ? 2 : ((3 * G_STAGE <= 96 * 1024) ? 3 : 2);
-  static constexpr int SMEM_BYTES = 1024 + A_STAGES * A_STAGE + G_STAGES * G_STAGE + 256;
+template <int BN>
+struct DwCfg {
+  static constexpr int G_TILE = BN * 128;
+  static constexpr int STAGE = 2 * DW_A_TILE + 2 * G_TILE;
+  static constexpr int SMEM_BYTES = 1024 + 2 * STAGE;
 };
 
-template <int BN, int OCC>
-__global__ void __launch_bounds__(DT_THREADS, OCC) ellconv_dw_tc_kernel(const __grid_constant__ DwTcParams p, int nct,
-                                                                      int tmem_cols, int split_roles) {
-  using Cfg = DtCfg<BN, OCC>;
-  constexpr int SA = Cfg::A_STAGES, SG = Cfg::G_STAGES;
+template <int BN>
+__global__ void __launch_bounds__(DW_THREADS, BN <= 64 ? 2 : 1) dw_wg_kernel(const __grid_constant__ DwTcParams p) {
+  using Cfg = DwCfg<BN>;
+  constexpr int NA = BN / 2;
+  constexpr int GQ = BN / 32;                // float4 column groups of G per thread
   extern __shared__ uint8_t smem_raw[];
   char* smem = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  char* a_ring = smem;
-  char* g_ring = smem + SA * Cfg::A_STAGE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(g_ring + SG * Cfg::G_STAGE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4 * DT_MAX_STAGES + 1);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = tid >> 7, wt = tid & 127;
   const int ftile = blockIdx.x * 128;
+  const int col0 = blockIdx.z * BN;
   const long long rbeg = (long long)blockIdx.y * p.rows_per_split;
   const long long rend = min(p.total_rows, rbeg + p.rows_per_split);
-  const uint32_t bar_afull = smem_u32(bars), bar_aempty = smem_u32(bars + DT_MAX_STAGES);
-  const uint32_t bar_gfull = smem_u32(bars + 2 * DT_MAX_STAGES), bar_gempty = smem_u32(bars + 3 * DT_MAX_STAGES);
-  const uint32_t bar_accum = smem_u32(bars + 4 * DT_MAX_STAGES);
+  const long long nchunks = (rend - rbeg + DW_KCH - 1) / DW_KCH;
 
-  if (warp == DT_PROD_WARPS) {
-    if (lane == 0) {
-      for (int s = 0; s < SA; ++s) { mbar_init(bar_afull + 8 * s, split_roles ? DT_PROD_WARPS / 2 : DT_PROD_WARPS); mbar_init(bar_aempty + 8 * s, 1); }
-      for (int s = 0; s < SG; ++s) { mbar_init(bar_gfull + 8 * s, split_roles ? DT_PROD_WARPS / 2 : DT_PROD_WARPS); mbar_init(bar_gempty + 8 * s, 1); }
-      mbar_init(bar_accum, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  float4 ra[4], rg[GQ];
+  // lane = row of the chunk; warp w covers the float4 groups w, w + 8, ... of f (A) and of c (G)
+  auto load_chunk = [&](long long kc) {
+    const long long R = rbeg + kc * DW_KCH + lane;
+    const bool live = R < rend;
+    const long long Q = live ? R : rbeg;
+    const int n = (int)(Q / p.rows_out), r = (int)(Q % p.rows_out);
+    const float* base = p.src + (size_t)n * p.src_rows * p.src_stride;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int f = ftile + 4 * (warp + 8 * i);
+      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (live && f < p.F) {
+        if (p.op.idx == nullptr) v = ldg4(base + (size_t)r * p.src_stride + f);
+        else ell_gather4(p.op, r, base + f, (size_t)p.src_stride, v);
+      }
+      ra[i] = v;
     }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const long long nchunks = (rend - rbeg + DT_KCH - 1) / DT_KCH;
+#pragma unroll
+    for (int i = 0; i < GQ; ++i) {
+      const int c = col0 + 4 * (warp + 8 * i);
+      rg[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (live && c < p.ncols) rg[i] = ldg4(p.g + (size_t)R * p.ncols + c);
+    }
+  };
+  auto store_chunk = [&](int stage) {
+    char* a_hi = smem + (size_t)stage * Cfg::STAGE;
+    char* a_lo = a_hi + DW_A_TILE;
+    char* g_hi = a_lo + DW_A_TILE;
+    char* g_lo = g_hi + Cfg::G_TILE;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int m = 4 * (warp + 8 * i);
+      split_store1(ra[i].x, a_hi, a_lo, sw_off(m, lane));
+      split_store1(ra[i].y, a_hi, a_lo, sw_off(m + 1, lane));
+      split_store1(ra[i].z, a_hi, a_lo, sw_off(m + 2, lane));
+      split_store1(ra[i].w, a_hi, a_lo, sw_off(m + 3, lane));
+    }
+#pragma unroll
+    for (int i = 0; i < GQ; ++i) {
+      const int m = 4 * (warp + 8 * i);
+      split_store1(rg[i].x, g_hi, g_lo, sw_off(m, lane));
+      split_store1(rg[i].y, g_hi, g_lo, sw_off(m + 1, lane));
+      split_store1(rg[i].z, g_hi, g_lo, sw_off(m + 2, lane));
+      split_store1(rg[i].w, g_hi, g_lo, sw_off(m + 3, lane));
+    }
+  };
 
-  if (warp < DT_PROD_WARPS) {
-    // =========================== producers ===========================
-    // Producer roles.  split_roles (wide outputs, ncols >= 256: the G stream is as heavy as the gather): warps 0-3
-    // gather the basis rows A, warps 4-7 stream the gradient rows G, concurrently, each running ahead as far as its
-    // ring allows.  Otherwise (narrow outputs: the gather dominates) all 8 warps do A and then G of each chunk.
-    const int mb = lane >> 3, ch = lane & 7;       // 32-element MN block and 16-byte chunk of this lane's float4
-    const int na = split_roles ? DT_PROD_WARPS / 2 : DT_PROD_WARPS;       // warps (and row stride) of the A group
-    const int ng = split_roles ? DT_PROD_WARPS / 2 : DT_PROD_WARPS;       // same for the G group
-    const bool do_a = !split_roles || warp < na;
-    const bool do_g = !split_roles || warp >= na;
-    const int wa = warp, wg = split_roles ? warp - na : warp;
-    int sa = 0, sg = 0;
-    uint32_t pha = 0, phg = 0;
-    const int fa = ftile + lane * 4;
-    const int cl = lane * 4;
-    for (long long kc = 0; kc < nchunks; ++kc) {
-      const long long rb = rbeg + kc * DT_KCH;
-      if (do_a) {
-        mbar_wait(bar_aempty + 8 * sa, pha ^ 1);
-        char* a_hi = a_ring + (size_t)sa * Cfg::A_STAGE;
-        char* a_lo = a_hi + DT_A_TILE;
-        for (int row_a = wa; row_a < DT_KCH; row_a += 2 * na) {
-          const int row_b = row_a + na;
-          const long long Ra = rb + row_a, Rb = rb + row_b;
-          float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (fa < p.F) {
-            // rows beyond the end of this split gather row 0 and are zeroed afterwards
-            const long long Qa = Ra < rend ? Ra : 0, Qb = Rb < rend ? Rb : 0;
-            const int n_a = (int)(Qa / p.rows_out), r_a = (int)(Qa % p.rows_out);
-            const int n_b = (int)(Qb / p.rows_out), r_b = (int)(Qb % p.rows_out);
-            const float* base_a = p.src + (size_t)n_a * p.src_rows * p.src_stride + fa;
-            const float* base_b = p.src + (size_t)n_b * p.src_rows * p.src_stride + fa;
-            if (p.op.idx == nullptr) {
-              va = ldg4(base_a + (size_t)r_a * p.src_stride);
-              vb = ldg4(base_b + (size_t)r_b * p.src_stride);
-            } else {
-              ell_gather4_pair(p.op, r_a, r_b, base_a, base_b, (size_t)p.src_stride, va, vb);
-            }
-            if (Ra >= rend) va = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (Rb >= rend) vb = make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-          split_store(va, a_hi, a_lo, mn_off(mb, row_a, ch));
-          split_store(vb, a_hi, a_lo, mn_off(mb, row_b, ch));
-        }
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_afull + 8 * sa);
-        if (++sa == SA) { sa = 0; pha ^= 1; }
-      }
-      if (do_g) {
-        for (int cs = 0; cs < nct; ++cs) {
-          mbar_wait(bar_gempty + 8 * sg, phg ^ 1);
-          char* g_hi = g_ring + (size_t)sg * Cfg::G_STAGE;
-          char* g_lo = g_hi + Cfg::G_TILE;
-          if (cl < BN) {
-            const int c = cs * BN + cl;
-            for (int r0 = wg; r0 < DT_KCH; r0 += 4 * ng) {            // 4 independent loads in flight per pass
-              float4 v[4];
+  float acc[NA];
 #pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const int row = r0 + i * ng;
-                const long long R = rb + row;
-                v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (row < DT_KCH && R < rend && c < p.ncols) v[i] = ldg4(p.g + (size_t)R * p.ncols + c);
-              }
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const int row = r0 + i * ng;
-                if (row < DT_KCH) split_store(v[i], g_hi, g_lo, mn_off(mb, row, ch));
-              }
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_gfull + 8 * sg);
-          if (++sg == SG) { sg = 0; phg ^= 1; }
-        }
-      }
-    }
+  for (int i = 0; i < NA; ++i) acc[i] = 0.f;
 
-    // =========================== epilogue: TMEM -> partial sums ===========================
-    mbar_wait(bar_accum, 0);
-    tc_fence_after();
-    const int quad = warp & 3, half = warp >> 2;
-    const int f = ftile + quad * 32 + lane;
-    const int cpw = p.ncols >> 1;
-    const uint32_t taddr_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-    float* orow = p.out + (p.nsplit > 1 ? (size_t)blockIdx.y * p.F * p.out_rs : 0) + (size_t)f * p.out_rs;
-#pragma unroll 1
-    for (int g = 0; g < cpw / 16; ++g) {
-      const int c0 = half * cpw + g * 16;
-      float v[16];
-      tmem_ld16(taddr_row + (uint32_t)c0, v);
-      if (f >= p.F) continue;
-      if (nchunks == 0) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) v[j] = 0.f;
+  if (nchunks > 0) {
+    load_chunk(0);
+    store_chunk(0);
+    fence_proxy_async();
+    __syncthreads();
+    for (long long kc = 0;; ++kc) {
+      const int stage = (int)(kc & 1);
+      const uint32_t base = smem_u32(smem + (size_t)stage * Cfg::STAGE);
+      const uint32_t a_hi = base + (uint32_t)(wgi * 64 * 128), a_lo = a_hi + DW_A_TILE;
+      const uint32_t g_hi = base + 2 * DW_A_TILE, g_lo = g_hi + Cfg::G_TILE;
+      wgmma_fence();
+      fence_acc(acc);
+      mma3_chunk<BN>(acc, a_hi, a_lo, g_hi, g_lo, 1);
+      wgmma_commit();
+      const bool more = kc + 1 < nchunks;
+      if (more) {
+        load_chunk(kc + 1);
+        store_chunk(stage ^ 1);
       }
-      if (p.nsplit == 1 && p.accumulate) {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) orow[c0 + j] += v[j];
-      } else if (p.ovec) {
-#pragma unroll
-        for (int j = 0; j < 16; j += 4)
-          *reinterpret_cast<float4*>(orow + c0 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 16; ++j) orow[c0 + j] = v[j];
-      }
+      wgmma_wait_all();
+      fence_acc(acc);
+      if (!more) break;
+      fence_proxy_async();
+      __syncthreads();
     }
-    tc_fence_before();
-  } else {
-    // =========================== MMA issuer (whole warp walks the loops, one elected lane issues) ===========================
-    {
-      // D=F32, A=B=TF32, A and B MN-major (bits 15,16), N=BN, M=128
-      constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | (1u << 15) | (1u << 16) |
-                                 ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      int sa = 0, sg = 0;
-      uint32_t pha = 0, phg = 0, acc_on = 0;
-      for (long long kc = 0; kc < nchunks; ++kc) {
-        mbar_wait(bar_afull + 8 * sa, pha);
-        const uint32_t aaddr = smem_u32(a_ring + (size_t)sa * Cfg::A_STAGE);
-        for (int cs = 0; cs < nct; ++cs) {
-          mbar_wait(bar_gfull + 8 * sg, phg);
-          tc_fence_after();
-          const uint32_t gaddr = smem_u32(g_ring + (size_t)sg * Cfg::G_STAGE);
-          const uint32_t d = tmem_base + (uint32_t)(cs * BN);
-          if (elect_one()) {
-#pragma unroll
-            for (int ks = 0; ks < DT_KCH / 8; ++ks) {
-              const uint64_t a_hi = make_desc_mn(aaddr + ks * 1024), a_lo = make_desc_mn(aaddr + DT_A_TILE + ks * 1024);
-              const uint64_t g_hi = make_desc_mn(gaddr + ks * 1024), g_lo = make_desc_mn(gaddr + Cfg::G_TILE + ks * 1024);
-              umma_tf32(d, a_hi, g_hi, idesc, ks == 0 ? acc_on : 1u);
-              umma_tf32(d, a_lo, g_hi, idesc, 1);
-              umma_tf32(d, a_hi, g_lo, idesc, 1);
-            }
-            umma_commit(bar_gempty + 8 * sg);
-            if (cs == nct - 1) umma_commit(bar_aempty + 8 * sa);
-          }
-          __syncwarp();
-          if (++sg == SG) { sg = 0; phg ^= 1; }
-        }
-        if (++sa == SA) { sa = 0; pha ^= 1; }
-        acc_on = 1;
-      }
-      if (elect_one()) umma_commit(bar_accum);
-    }
-    __syncwarp();
   }
 
-  __syncthreads();
-  if (warp == DT_PROD_WARPS) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols) : "memory");
+  // =========================== epilogue: accumulators -> dW or the split's partial sums ===========================
+  float* out = p.out + (p.nsplit > 1 ? (size_t)blockIdx.y * p.F * p.out_rs : 0);
+  const bool vec2 = (p.out_rs % 2 == 0) && ((reinterpret_cast<uintptr_t>(out) & 7u) == 0);
+#pragma unroll
+  for (int i = 0; i < NA; i += 2) {
+    const int f = ftile + wgi * 64 + frag_row(wt, i);
+    const int c = col0 + frag_col(wt, i);
+    if (f >= p.F || c >= p.ncols) continue;
+    float* o = out + (size_t)f * p.out_rs + c;
+    if (p.nsplit == 1 && p.accumulate) {
+      o[0] += acc[i];
+      o[1] += acc[i + 1];
+    } else if (vec2) {
+      *reinterpret_cast<float2*>(o) = make_float2(acc[i], acc[i + 1]);
+    } else {
+      o[0] = acc[i];
+      o[1] = acc[i + 1];
+    }
   }
 }
 
-template <int BN, int OCC>
+template <int BN>
 int launch_dw(const DwTcParams& p, int ftiles, cudaStream_t st) {
-  using Cfg = DtCfg<BN, OCC>;
+  using Cfg = DwCfg<BN>;
   static bool configured = false;
   if (!configured) {
-    CAPE_CHECK_CUDA(cudaFuncSetAttribute(ellconv_dw_tc_kernel<BN, OCC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES));
+    CAPE_CHECK_CUDA(cudaFuncSetAttribute(dw_wg_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     configured = true;
   }
-  const int nct = (p.ncols + BN - 1) / BN;
-  int cols = nct * BN, tmem_cols = 32;
-  while (tmem_cols < cols) tmem_cols *= 2;
-  dim3 grid(ftiles, p.nsplit);
-  ellconv_dw_tc_kernel<BN, OCC><<<grid, DT_THREADS, Cfg::SMEM_BYTES, st>>>(p, nct, tmem_cols, p.ncols >= 256 ? 1 : 0);
+  dim3 grid(ftiles, p.nsplit, (p.ncols + BN - 1) / BN);
+  dw_wg_kernel<BN><<<grid, DW_THREADS, Cfg::SMEM_BYTES, st>>>(p);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;
@@ -275,32 +176,33 @@ int launch_dw(const DwTcParams& p, int ftiles, cudaStream_t st) {
 int launch_ellconv_dw_tc(const cape_topology* t, const cape_dw_args* a, const OpView& op, int* nsplit_out,
                          cudaStream_t st) {
   if (!tensor_cores_enabled()) return 0;
-  if (a->ncols % 32 != 0 || a->ncols < 32 || a->ncols > 512 || (a->ncols > 128 && a->ncols % 128 != 0)) return 0;
+  if (a->ncols % 32 != 0 || a->ncols < 32 || a->ncols > 512) return 0;
   if (a->F % 4 != 0 || a->F < 32 || a->src_stride % 4 != 0 || !aligned16(a->src) || !aligned16(a->g)) return 0;
-  if (a->dw_stride % 4 != 0) { /* scalar stores are used anyway */ }
   DwTcParams p{};
   p.rows_out = a->rows_out; p.ncols = a->ncols; p.F = a->F; p.src_rows = a->src_rows; p.src_stride = a->src_stride;
   p.total_rows = (long long)a->N * a->rows_out;
-  if (p.total_rows < 4096) return 0;
+  if (p.total_rows < 4096 || p.total_rows >= (1LL << 31)) return 0;
   p.src = a->src; p.op = op; p.g = a->g;
-  const int ftiles = (a->F + 127) / 128;
-  long long nsplit = ((a->ncols >= 256 ? 2LL : 4LL) * t->sm_count + ftiles - 1) / ftiles;
+  const int BN = a->ncols <= 32 ? 32 : (a->ncols <= 64 ? 64 : (a->ncols <= 128 ? 128 : 256));
+  const int ftiles = (a->F + 127) / 128, ctiles = (a->ncols + BN - 1) / BN;
+  // about two waves of CTAs over the row splits
+  long long nsplit = (2LL * t->sm_count + ftiles * ctiles - 1) / (ftiles * ctiles);
   const long long max_by_rows = (p.total_rows + 511) / 512;
   if (nsplit > max_by_rows) nsplit = max_by_rows;
   const long long per = (long long)a->F * a->ncols * (long long)sizeof(float);
   if (nsplit > 1 && nsplit * per > t->workspace_bytes) nsplit = t->workspace_bytes / per;
   if (nsplit < 1) nsplit = 1;
   long long rps = (p.total_rows + nsplit - 1) / nsplit;
-  rps = (rps + DT_KCH - 1) / DT_KCH * DT_KCH;
+  rps = (rps + DW_KCH - 1) / DW_KCH * DW_KCH;
   nsplit = (p.total_rows + rps - 1) / rps;
   p.rows_per_split = rps; p.nsplit = (int)nsplit; p.accumulate = a->accumulate;
   if (nsplit == 1) { p.out = a->dw; p.out_rs = a->dw_stride; }
   else { p.out = (float*)t->workspace; p.out_rs = a->ncols; }
-  p.ovec = (p.out_rs % 4 == 0) && aligned16(p.out);
   *nsplit_out = (int)nsplit;
-  if (a->ncols >= 256) return launch_dw<128, 1>(p, ftiles, st);
-  if (a->ncols >= 64) return launch_dw<64, 2>(p, ftiles, st);    // 64-wide sub-tiles keep the G ring small
-  return launch_dw<32, 2>(p, ftiles, st);
+  if (BN == 32) return launch_dw<32>(p, ftiles, st);
+  if (BN == 64) return launch_dw<64>(p, ftiles, st);
+  if (BN == 128) return launch_dw<128>(p, ftiles, st);
+  return launch_dw<256>(p, ftiles, st);
 }
 
 }  // namespace cape

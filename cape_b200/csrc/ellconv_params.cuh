@@ -1,4 +1,4 @@
-// Parameter blocks shared by the SIMT (ellconv.cu) and tcgen05 (ellconv_tc.cu) fused-conv kernels.
+// Parameter blocks shared by the SIMT (ellconv.cu) and wgmma (ellconv_tc.cu) fused-conv kernels.
 #pragma once
 #include "common.cuh"
 
@@ -16,11 +16,11 @@ struct TermDev {
   int F, src_rows, src_stride, w_stride, w2_stride;
   const float* w;
   const float* w2;
-  const float* wT;    // K-major copy of w: element (f, c) = wT[c * wT_stride + f] (tcgen05 path), or nullptr
+  const float* wT;    // K-major copy of w: element (f, c) = wT[c * wT_stride + f] (tensor-core path), or nullptr
   const float* w2T;
   int wT_stride, w2T_stride;
   int vec;
-  const float* wT_lo;   // optional: wT - trunc_tf32(wT), same layout (weight tiles then come by TMA)
+  const float* wT_lo;   // optional: wT - trunc_tf32(wT), same layout (not read by the wgmma kernels)
   const float* w2T_lo;
   float* stash;       // optional copy of the gathered basis rows [total_rows, stash_stride] (cape_term.stash)
   int stash_stride;
@@ -45,14 +45,12 @@ struct ConvParams {
   float* out;
   float* out2;
   int wvec, ovec;
-  int split_rn;   // experiment (cape_set_tuning key 0): 0 = truncating 3xTF32 split, 1 = round to nearest, 2 = + lo*lo term
-  int precise;    // cape_conv_args.precise: split accumulation chains (gemm_tc.cu)
 };
 
 
-// all-plain-operand calls (every term an identity operator) on the TMA-fed kernel (gemm_tc.cu): 1 = launched, 0 = not eligible
+// all-plain-operand calls (every term an identity operator) on the wgmma kernel (ellconv_tc.cu): 1 = launched, 0 = not eligible
 int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st);
-// tcgen05 path (ellconv_tc.cu): returns 1 if it launched, 0 if the problem is not eligible, <0 on error.
+// wgmma path (ellconv_tc.cu): returns 1 if it launched, 0 if the problem is not eligible, <0 on error.
 int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st);
 bool tensor_cores_enabled();
 // thin-input layers (thin.cu): sources with <= 4 channels.  1 = launched, 0 = not eligible, <0 = error
@@ -61,18 +59,12 @@ int launch_thin_fwd(const cape_topology* t, const ConvParams& p, bool dual, cuda
 int launch_thinout_fwd(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st);
 int launch_thin_dw(const cape_topology* t, const cape_dw_args* a, const OpView* ops, int nops, int* nsplit_out,
                    cudaStream_t st);
-// tcgen05 weight-gradient path (ellconv_dw_tc.cu): 1 = launched (partials in the workspace if *nsplit_out > 1)
+// wgmma weight-gradient path (ellconv_dw_tc.cu), plain or gathered basis: 1 = launched (partials in the workspace if *nsplit_out > 1)
 int launch_ellconv_dw_tc(const cape_topology* t, const cape_dw_args* a, const OpView& op, int* nsplit_out,
                          cudaStream_t st);
 
-// dense-operand weight gradient on TMA + tcgen05 (dw_dense_tma.cu): same contract
-int launch_dw_dense_tma(const cape_topology* t, const cape_dw_args* a, const OpView& op, int* nsplit_out,
-                        cudaStream_t st);
-// experiment knobs (cape_set_tuning): [1] = 1 disables the TMA dense-dW kernel, [2] = its lo-part mode (1 = rna, wrong
-// on purpose: shows the tensor core truncates), [3] = 2: 128- instead of 256-wide G sub-tiles for wide outputs, [4] = 1: weight tiles of the wide conv kernel by the
-// producer warps instead of TMA, [5] = 1: one narrow-kernel CTA per SM (bigger L1), [6] = 1: identity-term basis
-// tiles by the producer warps instead of TMA, [7] = 1: thin-output layers on the generic kernels, [8] = 1: no TMA-fed
-// plain-operand kernel (gemm_tc.cu), [0]: operand-split experiment (ConvParams.split_rn)
+// experiment knobs (cape_set_tuning): [7] = 1: thin-output layers on the generic kernels, [8] = 1: no tensor-core
+// plain-operand path, [10]: rows per cape_apply CTA, [16] = 1: scalar FC kernel, [17] = 1: fixed thin-dW CTA count
 extern int g_tuning[32];
 
 }  // namespace cape

@@ -1,19 +1,21 @@
-// tcgen05 / TMEM version of the fused ELL-gather Chebyshev convolution (sm_100a only).
+// Tensor-core (wgmma, sm_90a) version of the fused ELL-gather Chebyshev convolution, and of the same contraction for
+// calls whose terms are all plain tensors (identity operators: 1x1 convs, the split convolution forms, the GroupNorm
+// blocks' linear layers).
 //
-// Same math and epilogues as ellconv.cu, but the [128 x Fin*K] x [Fin*K x BN] contraction runs on the 5th-gen
-// tensor cores with fp32 accuracy by 3xTF32 error compensation:  a = a_hi + a_lo (a_hi = top 19 bits, a_lo = the
-// exact remainder), acc += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo, fp32 accumulation in TMEM; the dropped a_lo*b_lo
-// term is ~2^-22 relative, so results stay within the 1e-4 parity gate with a wide margin.
+// Same math and epilogues as ellconv.cu, but the [128 x Fin*K] x [Fin*K x BN] contraction runs on the tensor cores
+// with fp32 accuracy by 3xTF32 error compensation:  a = a_hi + a_lo (a_hi = top 19 bits, a_lo = the exact remainder),
+// acc += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo with fp32 accumulation; the dropped a_lo*b_lo term is ~2^-22 relative.
 //
-// Persistent CTAs of 13 warps loop over 128-row output tiles (ALL output columns per tile).  Warps 0-7 build operand
-// tiles: the Chebyshev-basis chunk A[128 rows x 32 k] is gathered from neighbour rows with float4 loads (same ELL
-// tables as the SIMT path), split into hi/lo and written to shared memory in the canonical K-major SWIZZLE_128B
-// UMMA layout; the weight chunks B[BN x 32 k] (K-major copy of W) of every BN-wide column sub-tile are loaded and
-// split the same way.  Warp 8 issues tcgen05.mma (kind::tf32, M=128, N=BN, K=8; 12 per chunk and sub-tile, 24 for
-// the two-accumulator affine block) into one of two TMEM accumulator buffers and releases pipeline stages with
-// tcgen05.commit -> mbarrier.  Warps 9-12 are the epilogue: tcgen05.ld the finished accumulators, add the condition
-// broadcast / bias, apply the activation (or the affine-block / backward epilogues), store rows with float4
-// writes -- overlapping the next tile's main loop.
+// A CTA of two warpgroups owns one 128-row x BN-column output tile (grid.y walks the column tiles).  All 256 threads
+// gather the Chebyshev-basis chunk A[128 rows x 32 k] from neighbour rows (float4 loads, same ELL tables as the SIMT
+// path) and load the weight chunk B[BN x 32 k] (K-major copy of W), split both into hi/lo and store them in the
+// swizzled K-major layout; each warpgroup then issues wgmma m64nBNk8 for its 64 rows.  The shared-memory tiles are
+// double-buffered: the loads of chunk j+1 are in flight while the MMAs of chunk j run.
+//
+// Every chunk's products go to a fresh register accumulator that is added to the running sum in fp32 with
+// round-to-nearest, so the tensor core's truncating accumulation chain is one chunk (12 MMAs) long instead of the whole
+// reduction: long reductions would otherwise drift from the fp64 truth by more than 1e-4 (cape_conv_args.precise
+// has no effect).
 #include "common.cuh"
 #include "ellconv_params.cuh"
 #include "tc_common.cuh"
@@ -22,867 +24,267 @@ namespace cape {
 
 namespace {
 
-constexpr int TC_PROD_WARPS = 8;
-constexpr int TC_PROD_THREADS = TC_PROD_WARPS * 32;
-constexpr int TC_THREADS = TC_PROD_THREADS + 32;
-constexpr int A_TILE_BYTES = BM * 128;            // 128 rows x 32 fp32 (one 128-byte swizzle row each)
-constexpr int QS_FLOATS = 4096;
-constexpr int MAX_STAGES = 4;
-using namespace tc;     // mbarriers, fences, UMMA issue, TMEM loads, TMA loads (tc_common.cuh)
+using namespace tc;
 
-// K-major, SWIZZLE_128B shared-memory operand descriptor (cute::UMMA::SmemDescriptor, sm100 "version 1"):
-// start address >> 4 | LBO(ignored for swizzled K-major)=1 | SBO = 1024 B (8 rows x 128 B) | layout_type = 2.
-__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-
+constexpr int WG_THREADS = 256;
+constexpr int A_TILE = BM * 128;              // 128 rows x 32 fp32
+constexpr int QS_MAX_FLOATS = 8192;           // condition vectors of the tile's samples and columns
 
 template <int BN, bool DUAL>
-struct TcCfg {
-  static constexpr int B_TILE_BYTES = BN * 128;                       // one hi or lo tile of BN weight rows x 32 k
-  static constexpr int A_STAGE_BYTES = 2 * A_TILE_BYTES;              // hi + lo
-  static constexpr int B_STAGE_BYTES = (DUAL ? 4 : 2) * B_TILE_BYTES;  // hi + lo (+ second weight set)
-  static constexpr int A_STAGES = 2;
-  static constexpr int B_STAGES = (B_STAGE_BYTES * 3 <= 96 * 1024) ? 3 : 2;
-  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + A_STAGES * A_STAGE_BYTES + B_STAGES * B_STAGE_BYTES +
-                                    QS_FLOATS * 4 + 512;
+struct ConvCfg {
+  static constexpr int B_TILE = BN * 128;
+  static constexpr int STAGE = 2 * A_TILE + (DUAL ? 4 : 2) * B_TILE;
+  static constexpr int RING = 2 * STAGE;
 };
 
-constexpr int TC_EPI_WARPS = 4;
-constexpr int TC_EPI_WARP0 = TC_PROD_WARPS + 1;                        // warps 9..12: TMEM lane quadrants 1,2,3,0
-constexpr int TC_TMA_WARP = TC_EPI_WARP0 + TC_EPI_WARPS;               // warp 13: TMA issuer for the weight tiles
-constexpr int TC_THREADS3 = (TC_PROD_WARPS + 2 + TC_EPI_WARPS) * 32;   // 448
-constexpr int TC_TMA_TERMS = 4;
-
-// Tensor maps of the pre-split K-major weight copies, per term: [0] wT (raw fp32 = "hi": the tensor core reads the top
-// 19 bits), [1] wT_lo, [2] w2T, [3] w2T_lo.  Boxes of 32 k x BN columns, SWIZZLE_128B: a box lands as one operand tile.
-struct BMaps {
-  CUtensorMap m[TC_TMA_TERMS][4];
-  CUtensorMap a[TC_TMA_TERMS];     // identity-operator terms: the source rows themselves, boxes of 32 f x 128 rows
-};
-
-// Persistent kernel.  A CTA loops over 128-row output tiles (all output columns each).  Three roles run
-// concurrently on different tiles: 8 producer warps (gather/split/store the basis chunk A once per chunk, stream the
-// K-major weight chunks B of every BN-wide column sub-tile), 1 MMA warp (tcgen05.mma into one of TWO TMEM
-// accumulator buffers when 2 x accumulator columns <= 512), 4 epilogue warps (tcgen05.ld, condition/bias/
-// activation, stores) -- so the epilogue and start-up of one tile overlap the main loop of the next.
 template <int BN, bool DUAL>
-__global__ void __launch_bounds__(TC_THREADS3, 1) ellconv_tc_kernel(const __grid_constant__ ConvParams p,
-                                                                    const __grid_constant__ BMaps maps, int nct,
-                                                                    int tmem_cols, int nbuf, int ntiles, int tma_b, int tma_a) {
-  using Cfg = TcCfg<BN, DUAL>;
-  constexpr int SA = Cfg::A_STAGES, SB = Cfg::B_STAGES;
+__global__ void __launch_bounds__(WG_THREADS, BN <= 32 && !DUAL ? 2 : 1) conv_wg_kernel(const __grid_constant__ ConvParams p, int nqs) {
+  using Cfg = ConvCfg<BN, DUAL>;
+  constexpr int NA = BN / 2;                  // accumulator registers per thread
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment: required by SWIZZLE_128B operand tiles
   char* smem = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  char* a_ring = smem;
-  char* b_ring = smem + SA * Cfg::A_STAGE_BYTES;
-  float* qs_all = reinterpret_cast<float*>(b_ring + SB * Cfg::B_STAGE_BYTES);
-  // a_full[4] a_empty[4] b_full[4] b_empty[4] t_full[2] t_empty[2]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(qs_all + QS_FLOATS);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5 * MAX_STAGES + 4);
+  float* qs = reinterpret_cast<float*>(smem + Cfg::RING);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t bar_afull = smem_u32(bars), bar_aempty = smem_u32(bars + MAX_STAGES);
-  const uint32_t bar_bfull = smem_u32(bars + 2 * MAX_STAGES), bar_bempty = smem_u32(bars + 3 * MAX_STAGES);
-  const uint32_t bar_tfull = smem_u32(bars + 4 * MAX_STAGES), bar_tempty = smem_u32(bars + 4 * MAX_STAGES + 2);
-  const uint32_t bar_atma = smem_u32(bars + 4 * MAX_STAGES + 4);      // hi tile of an identity-term chunk landed (TMA)
-
-  if (warp == TC_PROD_WARPS) {
-    if (lane == 0) {
-      for (int s = 0; s < SA; ++s) { mbar_init(bar_afull + 8 * s, TC_PROD_WARPS); mbar_init(bar_aempty + 8 * s, 1); }
-      for (int s = 0; s < SB; ++s) {
-        mbar_init(bar_bfull + 8 * s, tma_b ? 1 : TC_PROD_WARPS);      // TMA: one arrive.expect_tx + the bytes
-        mbar_init(bar_bempty + 8 * s, 1);
-      }
-      for (int s = 0; s < 2; ++s) { mbar_init(bar_tfull + 8 * s, 1); mbar_init(bar_tempty + 8 * s, TC_EPI_WARPS); }
-      for (int s = 0; s < SA; ++s) mbar_init(bar_atma + 8 * s, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t acc1_col = (uint32_t)(nct * BN);            // second accumulator starts after the first
-  const uint32_t buf_cols = (uint32_t)((DUAL ? 2 : 1) * nct * BN);
-
-  if (warp < TC_PROD_WARPS) {
-    // =========================== producers ===========================
-    const int l8 = tid & 7, rs = tid >> 3;       // 8 lanes per 128-byte row, 32 row slots
-    int sa = 0, sb = 0;
-    uint32_t pha = 0, phb = 0, tph = 0;       // tph bit s: parity of the TMA fills stage s has seen (bar_atma)
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-      const long long row0 = (long long)tile * BM;
-      int rn[4], rr[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const long long R = row0 + rs + 32 * i;
-        if (R < p.total_rows) { rn[i] = (int)(R / p.rows_out); rr[i] = (int)(R % p.rows_out); }
-        else { rn[i] = -1; rr[i] = 0; }
-      }
-      for (int t = 0; t < p.nterms; ++t) {
-        const TermDev& tm = p.terms[t];
-        const bool has2 = DUAL && tm.w2T != nullptr;
-        for (int f0 = 0; f0 < tm.F; f0 += BK) {
-          const int f = f0 + l8 * 4;
-          // ---- issue the weight loads of the first column sub-tile now: they fly while the basis chunk is gathered
-          float4 bw[BN / 32], bw2[DUAL ? BN / 32 : 1];
-          auto load_b = [&](int cs) {
-#pragma unroll
-            for (int i = 0; i < BN / 32; ++i) {
-              const int c = cs * BN + rs + 32 * i;
-              bw[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (c < p.ncols && f < tm.F) bw[i] = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
-              if (DUAL) {
-                bw2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (has2 && c < p.ncols && f < tm.F) bw2[i] = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
-              }
-            }
-          };
-          if (!tma_b) load_b(0);
-          // ---- A chunk: gather 4 rows per thread, split, store swizzled
-          if ((tma_a >> t) & 1) {
-            // identity term: the TMA warp put the raw rows (= hi operand) in place; derive the lo tile from them
-            mbar_wait(bar_atma + 8 * sa, (tph >> sa) & 1u);
-            tph ^= 1u << sa;
-            char* a_hi = a_ring + (size_t)sa * Cfg::A_STAGE_BYTES;
-            char* a_lo = a_hi + A_TILE_BYTES;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const int row = rs + 32 * i;
-              const uint32_t off = (uint32_t)(row * 128 + ((l8 ^ (row & 7)) << 4));
-              const float4 v = *reinterpret_cast<const float4*>(a_hi + off);
-              float4 l;
-              l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xffffe000u);
-              l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xffffe000u);
-              l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xffffe000u);
-              l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xffffe000u);
-              *reinterpret_cast<float4*>(a_lo + off) = l;
-              if (tm.stash != nullptr && rn[i] >= 0 && f < tm.F)
-                *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row) * tm.stash_stride + f) = v;
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_afull + 8 * sa);
-            if (++sa == SA) { sa = 0; pha ^= 1; }
-          } else {
-          mbar_wait(bar_aempty + 8 * sa, pha ^ 1);
-          {
-            char* a_hi = a_ring + (size_t)sa * Cfg::A_STAGE_BYTES;
-            char* a_lo = a_hi + A_TILE_BYTES;
-#pragma unroll
-            for (int i = 0; i < 4; i += 2) {
-              const int row_a = rs + 32 * i, row_b = row_a + 32;
-              float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (f < tm.F) {
-                // invalid (beyond-the-end) rows gather sample 0 / row 0 and are zeroed afterwards
-                const float* base_a = tm.src + (size_t)max(rn[i], 0) * tm.src_rows * tm.src_stride + f;
-                const float* base_b = tm.src + (size_t)max(rn[i + 1], 0) * tm.src_rows * tm.src_stride + f;
-                if (tm.op.idx == nullptr) {
-                  va = ldg4(base_a + (size_t)rr[i] * tm.src_stride);
-                  vb = ldg4(base_b + (size_t)rr[i + 1] * tm.src_stride);
-                } else {
-                  ell_gather4_pair(tm.op, rr[i], rr[i + 1], base_a, base_b, (size_t)tm.src_stride, va, vb);
-                }
-                if (rn[i] < 0) va = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (rn[i + 1] < 0) vb = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (tm.stash != nullptr) {     // keep the basis rows for the weight gradient (cape_term.stash)
-                  if (rn[i] >= 0) *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row_a) * tm.stash_stride + f) = va;
-                  if (rn[i + 1] >= 0) *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row_b) * tm.stash_stride + f) = vb;
-                }
-              }
-              split_store(va, a_hi, a_lo, (uint32_t)(row_a * 128 + ((l8 ^ (row_a & 7)) << 4)));
-              split_store(vb, a_hi, a_lo, (uint32_t)(row_b * 128 + ((l8 ^ (row_b & 7)) << 4)));
-            }
-            fence_proxy_async();             // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_afull + 8 * sa);
-            if (++sa == SA) { sa = 0; pha ^= 1; }
-          }
-          }
-          // ---- B chunks: one [BN x 32] K-major weight tile (hi/lo) per column sub-tile (unless the TMA warp does it)
-          for (int cs = 0; cs < (tma_b ? 0 : nct); ++cs) {
-            if (cs > 0) load_b(cs);
-            mbar_wait(bar_bempty + 8 * sb, phb ^ 1);
-            char* b_hi = b_ring + (size_t)sb * Cfg::B_STAGE_BYTES;
-            char* b_lo = b_hi + Cfg::B_TILE_BYTES;
-#pragma unroll
-            for (int i = 0; i < BN / 32; ++i) {
-              const int cl = rs + 32 * i;
-              const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
-              split_store(bw[i], b_hi, b_lo, off);
-              if (DUAL) {
-                if (has2) split_store(bw2[i], b_lo + Cfg::B_TILE_BYTES, b_lo + 2 * Cfg::B_TILE_BYTES, off);
-              }
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_bfull + 8 * sb);
-            if (++sb == SB) { sb = 0; phb ^= 1; }
-          }
-        }
-      }
-    }
-  } else if (warp == TC_PROD_WARPS) {
-    // =========================== MMA issuer (whole warp walks the loops, one elected lane issues) ===========================
-    {
-      // instruction descriptor (cute::UMMA::InstrDescriptor): D=F32, A=B=TF32, both K-major, N=BN, M=128
-      constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int sa = 0, sb = 0, it = 0;
-      uint32_t pha = 0, phb = 0, tph = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const int buf = it % nbuf;
-        const uint32_t use = (uint32_t)(it / nbuf);
-        mbar_wait(bar_tempty + 8 * buf, (use & 1) ^ 1);       // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t tb = tmem_base + (uint32_t)buf * buf_cols;
-        uint32_t acc0_on = 0, acc1_on = 0;
-        for (int t = 0; t < p.nterms; ++t) {
-          const bool has2 = DUAL && p.terms[t].w2T != nullptr;
-          for (int f0 = 0; f0 < p.terms[t].F; f0 += BK) {
-            if ((tma_a >> t) & 1) { mbar_wait(bar_atma + 8 * sa, (tph >> sa) & 1u); tph ^= 1u << sa; }   // hi tile by TMA
-            mbar_wait(bar_afull + 8 * sa, pha);
-            const uint32_t aaddr = smem_u32(a_ring + (size_t)sa * Cfg::A_STAGE_BYTES);
-            const uint64_t a_hi = make_desc(aaddr), a_lo = make_desc(aaddr + A_TILE_BYTES);
-            for (int cs = 0; cs < nct; ++cs) {
-              mbar_wait(bar_bfull + 8 * sb, phb);
-              tc_fence_after();
-              const uint32_t baddr = smem_u32(b_ring + (size_t)sb * Cfg::B_STAGE_BYTES);
-              const uint64_t b_hi = make_desc(baddr), b_lo = make_desc(baddr + Cfg::B_TILE_BYTES);
-              const uint64_t b2_hi = make_desc(baddr + 2 * Cfg::B_TILE_BYTES), b2_lo = make_desc(baddr + 3 * Cfg::B_TILE_BYTES);
-              const uint32_t d0 = tb + (uint32_t)(cs * BN), d1 = d0 + acc1_col;
-              if (tc::elect_one()) {
-#pragma unroll
-                for (int ks = 0; ks < BK / 8; ++ks) {
-                  const uint64_t adv = (uint64_t)(ks * 2);  // +32 bytes along K inside the 128-byte swizzle row
-                  // the very first MMA into a sub-tile's TMEM columns overwrites (TMEM is not zero-initialised)
-                  umma_tf32(d0, a_hi + adv, b_hi + adv, idesc, ks == 0 ? acc0_on : 1u);
-                  umma_tf32(d0, a_lo + adv, b_hi + adv, idesc, 1);
-                  umma_tf32(d0, a_hi + adv, b_lo + adv, idesc, 1);
-                  if (has2) {
-                    umma_tf32(d1, a_hi + adv, b2_hi + adv, idesc, ks == 0 ? acc1_on : 1u);
-                    umma_tf32(d1, a_lo + adv, b2_hi + adv, idesc, 1);
-                    umma_tf32(d1, a_hi + adv, b2_lo + adv, idesc, 1);
-                  }
-                }
-                umma_commit(bar_bempty + 8 * sb);          // weight stage reusable once these MMAs have read it
-                if (cs == nct - 1) umma_commit(bar_aempty + 8 * sa);   // basis stage reusable
-              }
-              __syncwarp();
-              if (++sb == SB) { sb = 0; phb ^= 1; }
-            }
-            if (++sa == SA) { sa = 0; pha ^= 1; }
-            acc0_on = 1;
-            if (has2) acc1_on = 1;
-          }
-        }
-        if (tc::elect_one()) umma_commit(bar_tfull + 8 * buf);   // this tile's accumulators are complete
-        __syncwarp();
-      }
-    }
-    __syncwarp();
-  } else if (warp == TC_TMA_WARP) {
-    // =========================== TMA issuer: weight tiles (hi = raw fp32, lo = pre-split copy) ===========================
-    if (tma_b || tma_a) {
-      int sa = 0, sb = 0;
-      uint32_t pha = 0, phb = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-        const int row0 = tile * BM;
-        for (int t = 0; t < p.nterms; ++t) {
-          const bool has2 = DUAL && p.terms[t].w2T != nullptr;
-          const bool a_here = (tma_a >> t) & 1;
-          for (int f0 = 0; f0 < p.terms[t].F; f0 += BK) {
-            // Follow the A ring chunk by chunk even when the producers fill it: a parity wait cannot tell "two uses
-            // ago" from "this use", so this thread must never get more than one use of a stage ahead of the MMAs.
-            if (tma_a) mbar_wait(bar_aempty + 8 * sa, pha ^ 1);
-            if (a_here) {
-              if (tc::elect_one()) {
-                tc::mbar_arrive_expect_tx(bar_atma + 8 * sa, (uint32_t)A_TILE_BYTES);
-                tc::tma_load_2d(smem_u32(a_ring + (size_t)sa * Cfg::A_STAGE_BYTES), &maps.a[t], f0, row0, bar_atma + 8 * sa);
-              }
-              __syncwarp();
-            }
-            if (++sa == SA) { sa = 0; pha ^= 1; }
-            for (int cs = 0; cs < (tma_b ? nct : 0); ++cs) {
-              mbar_wait(bar_bempty + 8 * sb, phb ^ 1);
-              if (tc::elect_one()) {
-                tc::mbar_arrive_expect_tx(bar_bfull + 8 * sb, (uint32_t)((has2 ? 4 : 2) * Cfg::B_TILE_BYTES));
-                const uint32_t dst = smem_u32(b_ring + (size_t)sb * Cfg::B_STAGE_BYTES);
-                tc::tma_load_2d(dst, &maps.m[t][0], f0, cs * BN, bar_bfull + 8 * sb);
-                tc::tma_load_2d(dst + Cfg::B_TILE_BYTES, &maps.m[t][1], f0, cs * BN, bar_bfull + 8 * sb);
-                if (has2) {
-                  tc::tma_load_2d(dst + 2 * Cfg::B_TILE_BYTES, &maps.m[t][2], f0, cs * BN, bar_bfull + 8 * sb);
-                  tc::tma_load_2d(dst + 3 * Cfg::B_TILE_BYTES, &maps.m[t][3], f0, cs * BN, bar_bfull + 8 * sb);
-                }
-              }
-              __syncwarp();
-              if (++sb == SB) { sb = 0; phb ^= 1; }
-            }
-          }
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // =========================== epilogue warps ===========================
-    const int et = tid - TC_EPI_WARP0 * 32;               // 0..127
-    const int quad = warp & 3;                            // TMEM lane quadrant this warp may access
-    const int row = quad * 32 + lane;
-    int it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const int buf = it % nbuf;
-      const uint32_t use = (uint32_t)(it / nbuf);
-      const long long row0 = (long long)tile * BM;
-      const long long R = row0 + row;
-      const bool valid = R < p.total_rows;
-      const int n = valid ? (int)(R / p.rows_out) : -1, r = valid ? (int)(R % p.rows_out) : 0;
-      const int n_first = (int)(row0 / p.rows_out);
-      float* qs = qs_all + (size_t)(it & 1) * (QS_FLOATS / 2);   // always double-buffered (independent of nbuf)
-      if (p.nslots > 0) {
-        // condition broadcast vectors of this tile: q[s][slot][c] = cond[n_first+s,:] @ Wc_slot[:, c]
-        const long long rlast = min(p.total_rows, row0 + BM) - 1;
-        const int S = (int)(rlast / p.rows_out) - n_first + 1;
-        const int total = S * p.nslots * p.ncols;
-        for (int o = et; o < total; o += TC_EPI_WARPS * 32) {
-          const int c = o % p.ncols;
-          const int slot = (o / p.ncols) % p.nslots;
-          const int s = o / (p.ncols * p.nslots);
-          const float* y = p.cond + (size_t)(n_first + s) * p.C;
-          const float* wc = p.slot_w[slot] + c;
-          const int ws = p.slot_acc[slot] ? p.terms[p.slot_term[slot]].w2_stride : p.terms[p.slot_term[slot]].w_stride;
-          float q = 0.f;
-          for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * ws), q);
-          qs[o] = q;
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(TC_EPI_WARPS * 32) : "memory");
-      }
-      const size_t orow = (size_t)R * p.ncols;
-      // backward epilogues read the saved activation (aux), written a whole forward pass ago: while the MMAs of this
-      // tile run, pull this lane's row into L2 and start the first column group's loads; inside the loop the loads are
-      // fetched one column group ahead (they are row-strided, one row per lane)
-      const bool use_aux = valid && (p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK);
-      const float* bias_row = p.bias != nullptr ? p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) : nullptr;
-      const bool bias_vec = (reinterpret_cast<uintptr_t>(bias_row) & 15u) == 0;
-      float4 axn[4];
-      if (use_aux) {
-        for (int c = 0; c < p.ncols; c += 32) tc::prefetch_l2(p.aux + orow + c);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) axn[j] = ldg4(p.aux + orow + 4 * j);
-      }
-      mbar_wait(bar_tfull + 8 * buf, use & 1);
-      tc_fence_after();
-      const uint32_t taddr_row = tmem_base + (uint32_t)buf * buf_cols + ((uint32_t)(quad * 32) << 16);
-#pragma unroll 1
-      for (int c0 = 0; c0 < p.ncols; c0 += 16) {
-        float v0[16], v1[16];
-        float4 axc[4];
-        if (use_aux) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) axc[j] = axn[j];
-          if (c0 + 16 < p.ncols) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) axn[j] = ldg4(p.aux + orow + c0 + 16 + 4 * j);
-          }
-        }
-        tmem_ld16(taddr_row + (uint32_t)c0, v0);           // warp-collective: executed by every lane
-        if (DUAL) tmem_ld16(taddr_row + acc1_col + (uint32_t)c0, v1);
-        if (!valid) continue;
-        for (int slot = 0; slot < p.nslots; ++slot) {
-          const TermDev& tm = p.terms[p.slot_term[slot]];
-          const float coef = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
-          const float* q = qs + ((size_t)(n - n_first) * p.nslots + slot) * p.ncols + c0;
-          if (p.slot_acc[slot] == 0) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v0[j] = fmaf(coef, q[j], v0[j]);
-          } else if (DUAL) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) v1[j] = fmaf(coef, q[j], v1[j]);
-          }
-        }
-        float o1[16], o2[16];
-        bool write2 = false;
-        if (p.epilogue == CAPE_EPI_LINEAR) {
-          tc::bias_act16(v0, o1, bias_row != nullptr ? bias_row + c0 : nullptr, bias_vec, p.act, p.alpha);
-        } else if (p.epilogue == CAPE_EPI_AFFINE) {
-          write2 = p.out2 != nullptr;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float rg = fmaxf(v0[j], 0.f);
-            o1[j] = (DUAL ? v1[j] : 0.f) + rg;
-            o2[j] = rg;
-          }
-        } else {
-          float ax[16];
-#pragma unroll
-          for (int j = 0; j < 16; j += 4) {
-            const float4 a4 = axc[j >> 2];
-            ax[j] = a4.x; ax[j + 1] = a4.y; ax[j + 2] = a4.z; ax[j + 3] = a4.w;
-          }
-          if (p.epilogue == CAPE_EPI_SLOPE) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) o1[j] = v0[j] * (ax[j] > 0.f ? 1.f : p.alpha);
-          } else {
-            write2 = p.out2 != nullptr;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) { o1[j] = v0[j]; o2[j] = ax[j] > 0.f ? v0[j] : 0.f; }
-          }
-        }
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          *reinterpret_cast<float4*>(p.out + orow + c0 + j) = make_float4(o1[j], o1[j + 1], o1[j + 2], o1[j + 3]);
-          if (write2)
-            *reinterpret_cast<float4*>(p.out2 + orow + c0 + j) = make_float4(o2[j], o2[j + 1], o2[j + 2], o2[j + 3]);
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * buf);    // accumulator buffer free for the MMA warp
-    }
-  }
-
-  __syncthreads();
-  if (warp == TC_PROD_WARPS) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols) : "memory");
-  }
-}
-
-
-// K-major weight copy: element (f, c) at base[c * stride + f]; boxes of 32 f x bn columns, 128-byte swizzle
-bool make_wmap(CUtensorMap* m, const float* base, int F, int ncols, int stride, int bn) {
-  tc::EncodeTiledFn fn = tc::encode_fn();
-  if (!fn || base == nullptr || !aligned16(base) || stride % 4 != 0) return false;
-  const cuuint64_t dims[2] = {(cuuint64_t)F, (cuuint64_t)ncols};
-  const cuuint64_t strides[1] = {(cuuint64_t)stride * sizeof(float)};
-  const cuuint32_t box[2] = {32, (cuuint32_t)bn};
-  const cuuint32_t estr[2] = {1, 1};
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), dims, strides, box, estr,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// tensor maps of the pre-split weight copies of every term (cape_term.wT_lo); false: the producers load the weights
-template <bool DUAL>
-bool build_wmaps(const ConvParams& p, int bn, BMaps* maps) {
-  if (p.nterms > TC_TMA_TERMS) return false;
-  for (int i = 0; i < p.nterms; ++i) {
-    const TermDev& tm = p.terms[i];
-    if (tm.wT_lo == nullptr || (tm.w2T != nullptr && tm.w2T_lo == nullptr)) return false;
-    if (!make_wmap(&maps->m[i][0], tm.wT, tm.F, p.ncols, tm.wT_stride, bn) ||
-        !make_wmap(&maps->m[i][1], tm.wT_lo, tm.F, p.ncols, tm.wT_stride, bn))
-      return false;
-    if (DUAL && tm.w2T != nullptr) {
-      if (!make_wmap(&maps->m[i][2], tm.w2T, tm.F, p.ncols, tm.w2T_stride, bn) ||
-          !make_wmap(&maps->m[i][3], tm.w2T_lo, tm.F, p.ncols, tm.w2T_stride, bn))
-        return false;
-    }
-  }
-  return true;
-}
-
-template <int BN, bool DUAL>
-int launch_one(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
-  using Cfg = TcCfg<BN, DUAL>;
-  static bool configured = false;
-  if (!configured) {
-    CAPE_CHECK_CUDA(cudaFuncSetAttribute(ellconv_tc_kernel<BN, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES));
-    configured = true;
-  }
-  const int nct = (p.ncols + BN - 1) / BN;
-  const int acc_cols = (DUAL ? 2 : 1) * nct * BN;
-  const int nbuf = (2 * acc_cols <= 512) ? 2 : 1;
-  int tmem_cols = 32;
-  while (tmem_cols < acc_cols * nbuf) tmem_cols *= 2;
-  const int ntiles = (int)((p.total_rows + BM - 1) / BM);
-  const int grid = ntiles < t->sm_count ? ntiles : t->sm_count;
-  // weight tiles by TMA when every term comes with pre-split copies (cape_term.wT_lo)
-  static BMaps maps;                      // host-side scratch, copied into the launch
-  const int tma_b = g_tuning[4] != 1 && build_wmaps<DUAL>(p, BN, &maps);
-  // basis tiles of identity-operator terms (plain source rows) by TMA as well
-  int tma_a = 0;
-  if (tc::encode_fn() != nullptr && g_tuning[6] != 1 && p.total_rows < (1LL << 31)) {
-    for (int i = 0; i < p.nterms && i < TC_TMA_TERMS; ++i) {
-      const TermDev& tm = p.terms[i];
-      if (tm.op.idx != nullptr || tm.src_rows != p.rows_out || !tm.vec) continue;
-      tc::EncodeTiledFn fn = tc::encode_fn();
-      const cuuint64_t dims[2] = {(cuuint64_t)tm.F, (cuuint64_t)p.total_rows};
-      const cuuint64_t strides[1] = {(cuuint64_t)tm.src_stride * sizeof(float)};
-      const cuuint32_t box[2] = {32, (cuuint32_t)BM};
-      const cuuint32_t estr[2] = {1, 1};
-      if (fn(&maps.a[i], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(tm.src), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS)
-        tma_a |= 1 << i;
-    }
-  }
-  ellconv_tc_kernel<BN, DUAL><<<grid, TC_THREADS3, Cfg::SMEM_BYTES, st>>>(p, maps, nct, tmem_cols, nbuf, ntiles, tma_b,
-                                                                        tma_a);
-  CAPE_CHECK_CUDA(cudaGetLastError());
-  count_launches(1);
-  return 1;
-}
-
-constexpr int QS2_FLOATS = 2048;
-
-template <int BN, bool DUAL>
-struct Tc2Cfg {
-  static constexpr int B_TILE_BYTES = BN * 128;                       // one hi or lo tile of BN weight rows x 32 k
-  static constexpr int A_STAGE_BYTES = 2 * A_TILE_BYTES;              // hi + lo
-  static constexpr int B_STAGE_BYTES = (DUAL ? 4 : 2) * B_TILE_BYTES;  // hi + lo (+ second weight set)
-  static constexpr int A_STAGES = 2;
-  static constexpr int B_STAGES = 2;
-  static constexpr int SMEM_BYTES = 1024 /*align slack*/ + A_STAGES * A_STAGE_BYTES + B_STAGES * B_STAGE_BYTES +
-                                    QS2_FLOATS * 4 + 2 * BM * 4 + 256;
-};
-
-// Variant for NARROW outputs (accumulator <= 256 TMEM columns): one 128-row tile per CTA, 9 warps (the producer
-// warps double as the epilogue), <= 112 registers and ~106 KB of shared memory, so that TWO CTAs share an SM: twice
-// the warps hide the latency of the neighbour gather, and one CTA's epilogue overlaps the other's main loop.
-template <int BN, bool DUAL>
-__global__ void __launch_bounds__(TC_THREADS + 32, 2) ellconv_tc2_kernel(const __grid_constant__ ConvParams p,
-                                                                        const __grid_constant__ BMaps maps, int tma_b, int nct,
-                                                                   int tmem_cols) {
-  using Cfg = Tc2Cfg<BN, DUAL>;
-  constexpr int SA = Cfg::A_STAGES, SB = Cfg::B_STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment: required by SWIZZLE_128B operand tiles
-  char* smem = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  char* a_ring = smem;
-  char* b_ring = smem + SA * Cfg::A_STAGE_BYTES;
-  float* qs = reinterpret_cast<float*>(b_ring + SB * Cfg::B_STAGE_BYTES);
-  int* s_n = reinterpret_cast<int*>(qs + QS2_FLOATS);
-  int* s_r = s_n + BM;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_r + BM);   // a_full[4] a_empty[4] b_full[4] b_empty[4] accum
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4 * MAX_STAGES + 1);
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wgi = tid >> 7, wt = tid & 127;
   const long long row0 = (long long)blockIdx.x * BM;
-  const uint32_t bar_afull = smem_u32(bars), bar_aempty = smem_u32(bars + MAX_STAGES);
-  const uint32_t bar_bfull = smem_u32(bars + 2 * MAX_STAGES), bar_bempty = smem_u32(bars + 3 * MAX_STAGES);
-  const uint32_t bar_accum = smem_u32(bars + 4 * MAX_STAGES);
+  const int col0 = blockIdx.y * BN;
+  const int n_first = (int)(row0 / p.rows_out);
 
-  if (tid < BM) {
-    const long long R = row0 + tid;
-    if (R < p.total_rows) { s_n[tid] = (int)(R / p.rows_out); s_r[tid] = (int)(R % p.rows_out); }
-    else { s_n[tid] = -1; s_r[tid] = 0; }
-  }
-  if (warp == TC_PROD_WARPS) {
-    if (lane == 0) {
-      for (int s = 0; s < SA; ++s) { mbar_init(bar_afull + 8 * s, TC_PROD_WARPS); mbar_init(bar_aempty + 8 * s, 1); }
-      for (int s = 0; s < SB; ++s) { mbar_init(bar_bfull + 8 * s, tma_b ? 1 : TC_PROD_WARPS); mbar_init(bar_bempty + 8 * s, 1); }
-      mbar_init(bar_accum, 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)tmem_cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t acc1_col = (uint32_t)(nct * BN);            // second accumulator starts after the first
-
-  if (warp < TC_PROD_WARPS) {
-    // =========================== producers ===========================
-    const int l8 = tid & 7, rs = tid >> 3;       // 8 lanes per 128-byte row, 32 row slots
-    int sa = 0, sb = 0;
-    uint32_t pha = 0, phb = 0;
-    if (p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK) {
-      // the epilogue (these same warps, after the reduction) reads the saved activation of its row, written a whole
-      // forward pass ago: pull this lane's half row into L2 now
-      const int erow = (warp & 3) * 32 + lane, cpw = p.ncols >> 1;
-      if (s_n[erow] >= 0) {
-        const float* ap = p.aux + (size_t)(row0 + erow) * p.ncols + (warp >> 2) * cpw;
-        for (int c = 0; c < cpw; c += 32) tc::prefetch_l2(ap + c);
-      }
-    }
-    for (int t = 0; t < p.nterms; ++t) {
-      const TermDev& tm = p.terms[t];
-      const bool has2 = DUAL && tm.w2T != nullptr;
-      for (int f0 = 0; f0 < tm.F; f0 += BK) {
-        const int f = f0 + l8 * 4;
-        // ---- A chunk: gather 4 rows per thread, split, store swizzled
-        mbar_wait(bar_aempty + 8 * sa, pha ^ 1);
-        {
-          char* a_hi = a_ring + (size_t)sa * Cfg::A_STAGE_BYTES;
-          char* a_lo = a_hi + A_TILE_BYTES;
-#pragma unroll
-          for (int i = 0; i < 4; i += 2) {
-            const int row_a = rs + 32 * i, row_b = row_a + 32;
-            const int n_a = s_n[row_a], n_b = s_n[row_b];
-            float4 va = make_float4(0.f, 0.f, 0.f, 0.f), vb = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (f < tm.F) {
-              const float* base_a = tm.src + (size_t)max(n_a, 0) * tm.src_rows * tm.src_stride + f;
-              const float* base_b = tm.src + (size_t)max(n_b, 0) * tm.src_rows * tm.src_stride + f;
-              if (tm.op.idx == nullptr) {
-                va = ldg4(base_a + (size_t)s_r[row_a] * tm.src_stride);
-                vb = ldg4(base_b + (size_t)s_r[row_b] * tm.src_stride);
-              } else {
-                ell_gather4_pair(tm.op, s_r[row_a], s_r[row_b], base_a, base_b, (size_t)tm.src_stride, va, vb);
-              }
-              if (n_a < 0) va = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (n_b < 0) vb = make_float4(0.f, 0.f, 0.f, 0.f);
-              if (tm.stash != nullptr) {       // keep the basis rows for the weight gradient (cape_term.stash)
-                if (n_a >= 0) *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row_a) * tm.stash_stride + f) = va;
-                if (n_b >= 0) *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row_b) * tm.stash_stride + f) = vb;
-              }
-            }
-            split_store(va, a_hi, a_lo, (uint32_t)(row_a * 128 + ((l8 ^ (row_a & 7)) << 4)));
-            split_store(vb, a_hi, a_lo, (uint32_t)(row_b * 128 + ((l8 ^ (row_b & 7)) << 4)));
-          }
-          fence_proxy_async();               // generic-proxy smem writes -> visible to the tensor-core (async) proxy
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_afull + 8 * sa);
-          if (++sa == SA) { sa = 0; pha ^= 1; }
-        }
-        // ---- B chunks: one [BN x 32] K-major weight tile (hi/lo) per column sub-tile (unless the TMA warp does it)
-        for (int cs = 0; cs < (tma_b ? 0 : nct); ++cs) {
-          mbar_wait(bar_bempty + 8 * sb, phb ^ 1);
-          char* b_hi = b_ring + (size_t)sb * Cfg::B_STAGE_BYTES;
-          char* b_lo = b_hi + Cfg::B_TILE_BYTES;
-#pragma unroll
-          for (int i = 0; i < BN / 32; ++i) {
-            const int cl = rs + 32 * i;
-            const int c = cs * BN + cl;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (c < p.ncols && f < tm.F) v = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
-            const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
-            split_store(v, b_hi, b_lo, off);
-            if (DUAL) {
-              if (has2) {
-                float4 v2 = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (c < p.ncols && f < tm.F) v2 = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
-                split_store(v2, b_lo + Cfg::B_TILE_BYTES, b_lo + 2 * Cfg::B_TILE_BYTES, off);
-              }
-            }
-          }
-          fence_proxy_async();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_bfull + 8 * sb);
-          if (++sb == SB) { sb = 0; phb ^= 1; }
-        }
-      }
-    }
-
-    // ---- condition broadcast vectors: q[s][slot][c] = cond[n0+s,:] @ Wc_slot[:, c]
-    const int n_first = s_n[0];
-    if (p.nslots > 0) {
-      int n_last = n_first;
-      for (int i = BM - 1; i > 0; --i)
-        if (s_n[i] >= 0) { n_last = s_n[i]; break; }
-      const int S = n_last - n_first + 1;
-      const int total = S * p.nslots * p.ncols;
-      for (int o = tid; o < total; o += TC_PROD_THREADS) {
-        const int c = o % p.ncols;
-        const int slot = (o / p.ncols) % p.nslots;
-        const int s = o / (p.ncols * p.nslots);
-        const float* y = p.cond + (size_t)(n_first + s) * p.C;
-        const float* wc = p.slot_w[slot] + c;
+  // condition broadcast vectors of this tile: qs[s][slot][c] = cond[n_first + s, :] . Wc_slot[:, col0 + c]
+  if (p.nslots > 0) {
+    for (int o = tid; o < nqs; o += WG_THREADS) {
+      const int c = o % BN, slot = (o / BN) % p.nslots, s = o / (BN * p.nslots);
+      float q = 0.f;
+      const int n = n_first + s;
+      if (col0 + c < p.ncols && n < p.N) {
+        const float* y = p.cond + (size_t)n * p.C;
+        const float* wc = p.slot_w[slot] + col0 + c;
         const int ws = p.slot_acc[slot] ? p.terms[p.slot_term[slot]].w2_stride : p.terms[p.slot_term[slot]].w_stride;
-        float q = 0.f;
         for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * ws), q);
-        qs[o] = q;
       }
-      asm volatile("bar.sync 1, %0;" ::"n"(TC_PROD_THREADS) : "memory");
+      qs[o] = q;
     }
+  }
 
-    // =========================== epilogue ===========================
-    const int quad = warp & 3, half = warp >> 2;          // TMEM lane quadrant of this warp; column half
-    const int row = quad * 32 + lane;
-    const int n = s_n[row], r = s_r[row];
-    const int cpw = p.ncols >> 1;                         // columns per warp (ncols is a multiple of 32)
-    const uint32_t taddr_row = tmem_base + ((uint32_t)(quad * 32) << 16);
-    const size_t orow = (size_t)(row0 + row) * p.ncols;
-    // backward epilogues read the saved activation (aux): first column group before waiting for the MMAs, then one
-    // group ahead (row-strided loads, one row per lane: their latency would sit in front of every group)
-    const bool use_aux = n >= 0 && (p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK);
-    const float* bias_row = p.bias != nullptr ? p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) : nullptr;
-    const bool bias_vec = (reinterpret_cast<uintptr_t>(bias_row) & 15u) == 0;
-    float4 axn[4];
-    if (use_aux) {
+  // producer mapping: 8 threads per 128-byte tile row (one float4 of k each), 32 row slots
+  const int l8 = tid & 7, rs = tid >> 3;
+  int rn[4], rr[4];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) axn[j] = ldg4(p.aux + orow + half * cpw + 4 * j);
+  for (int i = 0; i < 4; ++i) {
+    const long long R = row0 + rs + 32 * i;
+    if (R < p.total_rows) { rn[i] = (int)(R / p.rows_out); rr[i] = (int)(R % p.rows_out); }
+    else { rn[i] = -1; rr[i] = 0; }
+  }
+  const bool do_stash = blockIdx.y == 0;      // one column tile writes the basis copies
+
+  float4 ra[4], rb[BN / 32], rb2[DUAL ? BN / 32 : 1];
+
+  auto load_chunk = [&](int t, int f0) {
+    const TermDev& tm = p.terms[t];
+    const int f = f0 + l8 * 4;
+#pragma unroll
+    for (int i = 0; i < 4; i += 2) {
+      float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (f < tm.F) {
+        // invalid (beyond-the-end) rows gather sample 0 / row 0 and are zeroed afterwards
+        const float* base_a = tm.src + (size_t)max(rn[i], 0) * tm.src_rows * tm.src_stride + f;
+        const float* base_b = tm.src + (size_t)max(rn[i + 1], 0) * tm.src_rows * tm.src_stride + f;
+        if (tm.op.idx == nullptr) {
+          a = ldg4(base_a + (size_t)rr[i] * tm.src_stride);
+          b = ldg4(base_b + (size_t)rr[i + 1] * tm.src_stride);
+        } else {
+          ell_gather4_pair(tm.op, rr[i], rr[i + 1], base_a, base_b, (size_t)tm.src_stride, a, b);
+        }
+        if (rn[i] < 0) a = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (rn[i + 1] < 0) b = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (tm.stash != nullptr && do_stash) {    // keep the basis rows for the weight gradient (cape_term.stash)
+          if (rn[i] >= 0) *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + rs + 32 * i) * tm.stash_stride + f) = a;
+          if (rn[i + 1] >= 0)
+            *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + rs + 32 * i + 32) * tm.stash_stride + f) = b;
+        }
+      }
+      ra[i] = a; ra[i + 1] = b;
     }
-    mbar_wait(bar_accum, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int g = 0; g < cpw / 16; ++g) {
-      const int c0 = half * cpw + g * 16;                 // first of 16 output columns
-      float v0[16], v1[16];
-      float4 axc[4];
-      if (use_aux) {
+    const bool has2 = DUAL && tm.w2T != nullptr;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) axc[j] = axn[j];
-        if (g + 1 < cpw / 16) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) axn[j] = ldg4(p.aux + orow + c0 + 16 + 4 * j);
-        }
+    for (int i = 0; i < BN / 32; ++i) {
+      const int c = col0 + rs + 32 * i;
+      rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (c < p.ncols && f < tm.F) rb[i] = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
+      if (DUAL) {
+        rb2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (has2 && c < p.ncols && f < tm.F) rb2[i] = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
       }
-      tmem_ld16(taddr_row + (uint32_t)c0, v0);             // warp-collective: executed by every lane
-      if (DUAL) tmem_ld16(taddr_row + acc1_col + (uint32_t)c0, v1);
-      if (n < 0) continue;
+    }
+  };
+  auto store_chunk = [&](int stage) {
+    char* a_hi = smem + (size_t)stage * Cfg::STAGE;
+    char* a_lo = a_hi + A_TILE;
+    char* b_hi = a_lo + A_TILE;
+    char* b_lo = b_hi + Cfg::B_TILE;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int row = rs + 32 * i;
+      split_store4(ra[i], a_hi, a_lo, (uint32_t)(row * 128 + ((l8 ^ (row & 7)) << 4)));
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 32; ++i) {
+      const int cl = rs + 32 * i;
+      const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
+      split_store4(rb[i], b_hi, b_lo, off);
+      if (DUAL) split_store4(rb2[i], b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, off);
+    }
+  };
+
+  float acc0[NA], acc1[DUAL ? NA : 1], part0[NA], part1[DUAL ? NA : 1];
+#pragma unroll
+  for (int i = 0; i < NA; ++i) { acc0[i] = 0.f; if (DUAL) acc1[i] = 0.f; }
+
+  // the reduction: 32-deep chunks over all terms
+  int t = 0, f0 = 0;
+  load_chunk(0, 0);
+  store_chunk(0);
+  fence_proxy_async();
+  __syncthreads();
+  for (int j = 0, stage = 0;; ++j, stage ^= 1) {
+    const uint32_t a_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + (uint32_t)(wgi * 64 * 128);
+    const uint32_t a_lo = a_hi + A_TILE;
+    const uint32_t b_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + 2 * A_TILE;
+    const uint32_t b_lo = b_hi + Cfg::B_TILE;
+    wgmma_fence();
+    fence_acc(part0);
+    mma3_chunk<BN>(part0, a_hi, a_lo, b_hi, b_lo, 0);
+    if constexpr (DUAL) {
+      fence_acc(part1);
+      mma3_chunk<BN>(part1, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
+    }
+    wgmma_commit();
+    // next chunk: its loads fly while the MMAs run; the other stage was released at the end of the previous pass
+    f0 += BK;
+    if (f0 >= p.terms[t].F) { f0 = 0; ++t; }
+    const bool more = t < p.nterms;
+    if (more) {
+      load_chunk(t, f0);
+      store_chunk(stage ^ 1);
+    }
+    wgmma_wait_all();
+    fence_acc(part0);
+#pragma unroll
+    for (int i = 0; i < NA; ++i) acc0[i] += part0[i];
+    if constexpr (DUAL) {
+      fence_acc(part1);
+#pragma unroll
+      for (int i = 0; i < NA; ++i) acc1[i] += part1[i];
+    }
+    if (!more) break;
+    fence_proxy_async();            // generic-proxy smem writes -> visible to the tensor core's (async) proxy
+    __syncthreads();                // both warpgroups done with this stage, the next one complete
+  }
+  __syncthreads();                  // qs complete (written before the main loop, read below)
+
+  // =========================== epilogue: straight from the accumulator registers ===========================
+  const bool linear = p.epilogue == CAPE_EPI_LINEAR;
+  const bool use_aux = p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {                       // the thread's two rows
+    const int lrow = wgi * 64 + frag_row(wt, 2 * h);
+    const long long R = row0 + lrow;
+    if (R >= p.total_rows) continue;
+    const int n = (int)(R / p.rows_out), r = (int)(R % p.rows_out);
+    const size_t orow = (size_t)R * p.ncols;
+    float coef[MAX_SLOTS];
+    for (int slot = 0; slot < p.nslots; ++slot) {
+      const TermDev& tm = p.terms[p.slot_term[slot]];
+      coef[slot] = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
+    }
+    const float* bias_row = (linear && p.bias != nullptr) ? p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) : nullptr;
+#pragma unroll
+    for (int g = 0; g < NA / 4; ++g) {
+      const int i = 4 * g + 2 * h;
+      const int c = col0 + frag_col(wt, i);
+      if (c >= p.ncols) continue;
+      float v0[2] = {acc0[i], acc0[i + 1]}, v1[2] = {0.f, 0.f};
+      if (DUAL) { v1[0] = acc1[i]; v1[1] = acc1[i + 1]; }
       for (int slot = 0; slot < p.nslots; ++slot) {
-        const TermDev& tm = p.terms[p.slot_term[slot]];
-        const float coef = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
-        const float* q = qs + ((size_t)(n - n_first) * p.nslots + slot) * p.ncols + c0;
+        const float* q = qs + ((size_t)(n - n_first) * p.nslots + slot) * BN + (c - col0);
         if (p.slot_acc[slot] == 0) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v0[j] = fmaf(coef, q[j], v0[j]);
+          v0[0] = fmaf(coef[slot], q[0], v0[0]); v0[1] = fmaf(coef[slot], q[1], v0[1]);
         } else if (DUAL) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v1[j] = fmaf(coef, q[j], v1[j]);
+          v1[0] = fmaf(coef[slot], q[0], v1[0]); v1[1] = fmaf(coef[slot], q[1], v1[1]);
         }
       }
-      float o1[16], o2[16];
+      float o1[2], o2[2];
       bool write2 = false;
-      if (p.epilogue == CAPE_EPI_LINEAR) {
-        tc::bias_act16(v0, o1, bias_row != nullptr ? bias_row + c0 : nullptr, bias_vec, p.act, p.alpha);
+      if (linear) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float v = v0[e] + (bias_row != nullptr ? __ldg(bias_row + c + e) : 0.f);
+          if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
+          else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
+          o1[e] = v;
+        }
       } else if (p.epilogue == CAPE_EPI_AFFINE) {
         write2 = p.out2 != nullptr;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const float rg = fmaxf(v0[j], 0.f);
-          o1[j] = (DUAL ? v1[j] : 0.f) + rg;
-          o2[j] = rg;
+        for (int e = 0; e < 2; ++e) {
+          const float rg = fmaxf(v0[e], 0.f);
+          o1[e] = (DUAL ? v1[e] : 0.f) + rg;
+          o2[e] = rg;
         }
       } else {
-        float ax[16];
-#pragma unroll
-        for (int j = 0; j < 16; j += 4) {
-          const float4 a4 = axc[j >> 2];
-          ax[j] = a4.x; ax[j + 1] = a4.y; ax[j + 2] = a4.z; ax[j + 3] = a4.w;
-        }
+        const float2 ax = use_aux ? __ldg(reinterpret_cast<const float2*>(p.aux + orow + c)) : make_float2(0.f, 0.f);
+        const float a2[2] = {ax.x, ax.y};
         if (p.epilogue == CAPE_EPI_SLOPE) {
 #pragma unroll
-          for (int j = 0; j < 16; ++j) o1[j] = v0[j] * (ax[j] > 0.f ? 1.f : p.alpha);
+          for (int e = 0; e < 2; ++e) o1[e] = v0[e] * (a2[e] > 0.f ? 1.f : p.alpha);
         } else {
           write2 = p.out2 != nullptr;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) { o1[j] = v0[j]; o2[j] = ax[j] > 0.f ? v0[j] : 0.f; }
+          for (int e = 0; e < 2; ++e) { o1[e] = v0[e]; o2[e] = a2[e] > 0.f ? v0[e] : 0.f; }
         }
       }
-#pragma unroll
-      for (int j = 0; j < 16; j += 4) {
-        *reinterpret_cast<float4*>(p.out + orow + c0 + j) = make_float4(o1[j], o1[j + 1], o1[j + 2], o1[j + 3]);
-        if (write2)
-          *reinterpret_cast<float4*>(p.out2 + orow + c0 + j) = make_float4(o2[j], o2[j + 1], o2[j + 2], o2[j + 3]);
-      }
+      *reinterpret_cast<float2*>(p.out + orow + c) = make_float2(o1[0], o1[1]);
+      if (write2) *reinterpret_cast<float2*>(p.out2 + orow + c) = make_float2(o2[0], o2[1]);
     }
-    tc_fence_before();
-  } else if (warp == TC_PROD_WARPS + 1) {
-    // =========================== TMA issuer: weight tiles (hi = raw fp32, lo = pre-split copy) ===========================
-    if (tma_b) {
-      int sb = 0;
-      uint32_t phb = 0;
-      for (int t = 0; t < p.nterms; ++t) {
-        const bool has2 = DUAL && p.terms[t].w2T != nullptr;
-        for (int f0 = 0; f0 < p.terms[t].F; f0 += BK) {
-          for (int cs = 0; cs < nct; ++cs) {
-            mbar_wait(bar_bempty + 8 * sb, phb ^ 1);
-            if (tc::elect_one()) {
-              tc::mbar_arrive_expect_tx(bar_bfull + 8 * sb, (uint32_t)((has2 ? 4 : 2) * Cfg::B_TILE_BYTES));
-              const uint32_t dst = smem_u32(b_ring + (size_t)sb * Cfg::B_STAGE_BYTES);
-              tc::tma_load_2d(dst, &maps.m[t][0], f0, cs * BN, bar_bfull + 8 * sb);
-              tc::tma_load_2d(dst + Cfg::B_TILE_BYTES, &maps.m[t][1], f0, cs * BN, bar_bfull + 8 * sb);
-              if (has2) {
-                tc::tma_load_2d(dst + 2 * Cfg::B_TILE_BYTES, &maps.m[t][2], f0, cs * BN, bar_bfull + 8 * sb);
-                tc::tma_load_2d(dst + 3 * Cfg::B_TILE_BYTES, &maps.m[t][3], f0, cs * BN, bar_bfull + 8 * sb);
-              }
-            }
-            __syncwarp();
-            if (++sb == SB) { sb = 0; phb ^= 1; }
-          }
-        }
-      }
-    }
-    __syncwarp();
-  } else {
-    // =========================== MMA issuer (whole warp walks the loops, one elected lane issues) ===========================
-    {
-      // instruction descriptor (cute::UMMA::InstrDescriptor): D=F32, A=B=TF32, both K-major, N=BN, M=128
-      constexpr uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-      int sa = 0, sb = 0;
-      uint32_t pha = 0, phb = 0, acc0_on = 0, acc1_on = 0;
-      for (int t = 0; t < p.nterms; ++t) {
-        const bool has2 = DUAL && p.terms[t].w2T != nullptr;
-        for (int f0 = 0; f0 < p.terms[t].F; f0 += BK) {
-          mbar_wait(bar_afull + 8 * sa, pha);
-          const uint32_t aaddr = smem_u32(a_ring + (size_t)sa * Cfg::A_STAGE_BYTES);
-          const uint64_t a_hi = make_desc(aaddr), a_lo = make_desc(aaddr + A_TILE_BYTES);
-          for (int cs = 0; cs < nct; ++cs) {
-            mbar_wait(bar_bfull + 8 * sb, phb);
-            tc_fence_after();
-            const uint32_t baddr = smem_u32(b_ring + (size_t)sb * Cfg::B_STAGE_BYTES);
-            const uint64_t b_hi = make_desc(baddr), b_lo = make_desc(baddr + Cfg::B_TILE_BYTES);
-            const uint64_t b2_hi = make_desc(baddr + 2 * Cfg::B_TILE_BYTES), b2_lo = make_desc(baddr + 3 * Cfg::B_TILE_BYTES);
-            const uint32_t d0 = tmem_base + (uint32_t)(cs * BN), d1 = d0 + acc1_col;
-            if (tc::elect_one()) {
-#pragma unroll
-              for (int ks = 0; ks < BK / 8; ++ks) {
-                const uint64_t adv = (uint64_t)(ks * 2);  // +32 bytes along K inside the 128-byte swizzle row
-                // the very first MMA into a sub-tile's TMEM columns overwrites (TMEM is not zero-initialised)
-                umma_tf32(d0, a_hi + adv, b_hi + adv, idesc, ks == 0 ? acc0_on : 1u);
-                umma_tf32(d0, a_lo + adv, b_hi + adv, idesc, 1);
-                umma_tf32(d0, a_hi + adv, b_lo + adv, idesc, 1);
-                if (has2) {
-                  umma_tf32(d1, a_hi + adv, b2_hi + adv, idesc, ks == 0 ? acc1_on : 1u);
-                  umma_tf32(d1, a_lo + adv, b2_hi + adv, idesc, 1);
-                  umma_tf32(d1, a_hi + adv, b2_lo + adv, idesc, 1);
-                }
-              }
-              umma_commit(bar_bempty + 8 * sb);            // weight stage reusable once these MMAs have read it
-              if (cs == nct - 1) umma_commit(bar_aempty + 8 * sa);     // basis stage reusable
-            }
-            __syncwarp();
-            if (++sb == SB) { sb = 0; phb ^= 1; }
-          }
-          if (++sa == SA) { sa = 0; pha ^= 1; }
-          acc0_on = 1;
-          if (has2) acc1_on = 1;
-        }
-      }
-      if (tc::elect_one()) umma_commit(bar_accum);         // accumulators complete
-    }
-    __syncwarp();
-  }
-
-  __syncthreads();
-  if (warp == TC_PROD_WARPS) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)tmem_cols) : "memory");
   }
 }
 
 template <int BN, bool DUAL>
-int launch_two(const ConvParams& p, cudaStream_t st) {
-  using Cfg = Tc2Cfg<BN, DUAL>;
+int launch_conv(const ConvParams& p, cudaStream_t st) {
+  using Cfg = ConvCfg<BN, DUAL>;
+  int nqs = 0;
+  if (p.nslots > 0) {
+    const long long rlast_max = BM - 1;
+    const int S = (int)(rlast_max / p.rows_out) + 2;
+    nqs = S * p.nslots * BN;
+  }
+  const int smem = 1024 + Cfg::RING + nqs * 4;
   static bool configured = false;
   if (!configured) {
-    CAPE_CHECK_CUDA(cudaFuncSetAttribute(ellconv_tc2_kernel<BN, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES + 24 * 1024));
+    CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         1024 + Cfg::RING + QS_MAX_FLOATS * 4));
     configured = true;
   }
-  const int nct = (p.ncols + BN - 1) / BN;
-  int cols = (DUAL ? 2 : 1) * nct * BN, tmem_cols = 32;
-  while (tmem_cols < cols) tmem_cols *= 2;
-  dim3 grid((unsigned)((p.total_rows + BM - 1) / BM), 1);
-  // experiment [5] = 1: pad the request so that only one CTA fits per SM and the L1 gets the rest
-  const int smem = Cfg::SMEM_BYTES + (g_tuning[5] == 1 ? 24 * 1024 : 0);
-  static BMaps maps;
-  const int tma_b = g_tuning[4] != 1 && build_wmaps<DUAL>(p, BN, &maps);
-  ellconv_tc2_kernel<BN, DUAL><<<grid, TC_THREADS + 32, smem, st>>>(p, maps, tma_b, nct, tmem_cols);
+  dim3 grid((unsigned)((p.total_rows + BM - 1) / BM), (unsigned)((p.ncols + BN - 1) / BN));
+  conv_wg_kernel<BN, DUAL><<<grid, WG_THREADS, smem, st>>>(p, nqs);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;
+}
+
+// column tile width: the whole output row up to 128 columns (64 with two accumulators), so that the running sums and
+// the chunk accumulators fit the registers
+int pick_bn(int ncols, bool dual) {
+  if (ncols <= 32) return 32;
+  if (ncols <= 64 || dual) return 64;
+  return 128;
+}
+
+// false if the condition vectors of a tile would not fit the staging buffer
+bool qs_fits(const ConvParams& p, int bn) {
+  if (p.nslots == 0) return true;
+  const long long max_samples = (BM - 1) / p.rows_out + 2;
+  return max_samples * p.nslots * bn <= QS_MAX_FLOATS;
 }
 
 }  // namespace
@@ -892,36 +294,49 @@ int g_tuning[32] = {0};   // experiment knobs (cape_set_tuning), see ellconv_par
 bool tensor_cores_enabled() { return g_tc_enabled; }
 
 int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
+  (void)t;
   if (!g_tc_enabled) return 0;
   if (p.ncols % 32 != 0 || p.ncols < 32 || !p.ovec) return 0;
-  if ((dual ? 2 : 1) * p.ncols > 512) return 0;              // the whole accumulator row must fit the 512 TMEM columns
-  if (p.ncols > 128 && p.ncols % 128 != 0) return 0;
+  if ((dual ? 2 : 1) * p.ncols > 512) return 0;
   long long kred = 0;
   for (int i = 0; i < p.nterms; ++i) {
     const TermDev& tm = p.terms[i];
     if (!tm.vec || tm.wT == nullptr || (tm.wT_stride % 4) != 0 || !aligned16(tm.wT)) return 0;
     if (tm.w2 != nullptr && (tm.w2T == nullptr || (tm.w2T_stride % 4) != 0 || !aligned16(tm.w2T))) return 0;
+    if (tm.stash != nullptr && (tm.stash_stride % 4) != 0) return 0;
     kred += tm.F;
   }
   if (kred < 64) return 0;                       // tiny reductions: the SIMT kernel is as good and simpler
-  if (p.nslots > 0) {
-    const long long max_samples = (BM - 1) / p.rows_out + 2;
-    if (max_samples * p.nslots * p.ncols > QS_FLOATS / 2) return 0;
+  const int bn = pick_bn(p.ncols, dual);
+  if (!qs_fits(p, bn)) return 0;
+  if (dual) return bn == 32 ? launch_conv<32, true>(p, st) : launch_conv<64, true>(p, st);
+  if (bn == 32) return launch_conv<32, false>(p, st);
+  if (bn == 64) return launch_conv<64, false>(p, st);
+  return launch_conv<128, false>(p, st);
+}
+
+// all-plain-operand calls: 1 = launched, 0 = not eligible (the caller falls through to the gather kernels)
+int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
+  (void)t;
+  if (!tensor_cores_enabled() || g_tuning[8] == 1) return 0;
+  if (dual || p.epilogue == CAPE_EPI_AFFINE) return 0;
+  if (p.ncols % 16 != 0 || p.ncols < 32 || !p.ovec) return 0;
+  if (p.total_rows >= (1LL << 31)) return 0;
+  long long kred = 0;
+  for (int i = 0; i < p.nterms; ++i) {
+    const TermDev& tm = p.terms[i];
+    if (tm.op.idx != nullptr || tm.src_rows != p.rows_out || !tm.vec || tm.stash != nullptr) return 0;
+    if (tm.wT == nullptr || (tm.wT_stride % 4) != 0 || !aligned16(tm.wT)) return 0;
+    kred += tm.F;
   }
-  // narrow outputs: accumulator <= 128 TMEM columns -> the two-CTAs-per-SM variant (wider ones measured slower)
-  if ((dual ? 2 : 1) * p.ncols <= 128 && (!p.nslots || (long long)((BM - 1) / p.rows_out + 2) * p.nslots * p.ncols <= QS2_FLOATS)) {
-    if (dual) return launch_two<32, true>(p, st);      // 32-wide sub-tiles: two weight sets per stage must stay small
-    if (p.ncols >= 64) return launch_two<64, false>(p, st);
-    return launch_two<32, false>(p, st);
-  }
-  if (dual) {
-    if (p.ncols >= 128) return launch_one<128, true>(t, p, st);
-    if (p.ncols >= 64) return launch_one<64, true>(t, p, st);
-    return launch_one<32, true>(t, p, st);
-  }
-  if (p.ncols >= 128) return launch_one<128, false>(t, p, st);
-  if (p.ncols >= 64) return launch_one<64, false>(t, p, st);
-  return launch_one<32, false>(t, p, st);
+  if (kred < 32) return 0;
+  for (int s = 0; s < p.nslots; ++s)
+    if (p.slot_acc[s] != 0) return 0;
+  const int bn = pick_bn(p.ncols, false);
+  if (!qs_fits(p, bn)) return 0;
+  if (bn == 32) return launch_conv<32, false>(p, st);
+  if (bn == 64) return launch_conv<64, false>(p, st);
+  return launch_conv<128, false>(p, st);
 }
 
 }  // namespace cape

@@ -1,7 +1,7 @@
 // Strided fp32 GEMM with deterministic split-K: the dense layers of CAPE
 // (tf.layers.dense at lib/models.py:496,506,510,557,560,582) and their gradients.
 // These are weight-bandwidth bound (2 x 55168x64 + 128x55168 fp32 = 56.7 MB read once per pass at batch 64),
-// so the contraction stays on the fp32 pipe; split-K over the 55168-long reduction fills the 148 SMs.
+// so the contraction stays on the fp32 pipe; split-K over the 55168-long reduction fills the SMs.
 #include "common.cuh"
 #include "ellconv_params.cuh"
 

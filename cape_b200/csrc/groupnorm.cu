@@ -194,7 +194,7 @@ extern "C" int cape_gn_relu_fwd(cape_topology* t, const float* x, int N, int row
   cape::count_launches(1);
   {
     long long bx = ((long long)rows * (C / 4) + 255) / 256;
-    const long long cap = (148LL * 16 + N - 1) / N;
+    const long long cap = ((long long)H100_SMS * 16 + N - 1) / N;
     if (bx > cap) bx = cap;
     gn_apply_kernel<<<dim3((unsigned)bx, (unsigned)N), 256, 0, st>>>(x, rows, C, G, gamma, beta, stats, y);
   }
@@ -218,7 +218,7 @@ extern "C" int cape_gn_relu_bwd(cape_topology* t, const float* x, const float* y
   const double inv_cnt = 1.0 / ((double)rows * (C / G));
   {
     long long bx = ((long long)rows * (C / 4) + 255) / 256;
-    const long long cap = (148LL * 16 + N - 1) / N;
+    const long long cap = ((long long)H100_SMS * 16 + N - 1) / N;
     if (bx > cap) bx = cap;
     gn_bwd_apply_kernel<<<dim3((unsigned)bx, (unsigned)N), 256, 0, st>>>(x, y, dy, rows, C, G, gamma, stats, acc, inv_cnt, dx,
                                                                          accumulate_dx);

@@ -142,7 +142,7 @@ __global__ void bce_kernel(const float* __restrict__ logits, long long n, float 
 // Deterministic: block partial sums go to a scratch array and the LAST block to finish adds them up in index order, so
 // the global norm (and with it the clip factor of the update) is bit-identical on every data-parallel replica and in
 // every run -- a float atomicAdd per block is not, and replicas that clip would drift apart by an ulp per step.
-constexpr int SUMSQ_MAX_BLOCKS = 148 * 4;
+constexpr int SUMSQ_MAX_BLOCKS = H100_SMS * 4;
 __device__ float g_sumsq_partials[SUMSQ_MAX_BLOCKS];
 __device__ unsigned int g_sumsq_counter = 0;
 
@@ -312,7 +312,7 @@ using namespace cape;
 
 extern "C" int cape_act_bwd(const float* dy, const float* y, float* g, int64_t n, float alpha, void* stream) {
   CAPE_REQUIRE(dy && y && g && n > 0, "bad arguments");
-  act_bwd_kernel<<<blocks_for(n, 256, 148 * 8), 256, 0, (cudaStream_t)stream>>>(dy, y, g, n, alpha);
+  act_bwd_kernel<<<blocks_for(n, 256, H100_SMS * 8), 256, 0, (cudaStream_t)stream>>>(dy, y, g, n, alpha);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   return 0;
@@ -320,7 +320,7 @@ extern "C" int cape_act_bwd(const float* dy, const float* y, float* g, int64_t n
 
 extern "C" int cape_axpy(float* y, const float* x, float a, int64_t n, void* stream) {
   CAPE_REQUIRE(y && x && n > 0, "bad arguments");
-  axpy_kernel<<<blocks_for(n, 256, 148 * 8), 256, 0, (cudaStream_t)stream>>>(y, x, a, n);
+  axpy_kernel<<<blocks_for(n, 256, H100_SMS * 8), 256, 0, (cudaStream_t)stream>>>(y, x, a, n);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   return 0;
@@ -397,7 +397,7 @@ extern "C" int cape_sumsq(const float* g, int64_t n, float* sumsq, void* stream)
 extern "C" int cape_sgd_clip_update(float* w, const float* g, float* mom, int64_t n, const float* sumsq,
                                     float clip_norm, const float* lr_dev, float momentum, void* stream) {
   CAPE_REQUIRE(w && g && mom && lr_dev && n > 0, "bad arguments");
-  sgd_kernel<<<blocks_for(n, 256, 148 * 8), 256, 0, (cudaStream_t)stream>>>(w, g, mom, n, sumsq, clip_norm, lr_dev,
+  sgd_kernel<<<blocks_for(n, 256, H100_SMS * 8), 256, 0, (cudaStream_t)stream>>>(w, g, mom, n, sumsq, clip_norm, lr_dev,
                                                                              momentum);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
@@ -409,7 +409,7 @@ extern "C" int cape_adam_clip_update(float* w, const float* g, float* m, float* 
                                      void* stream) {
   CAPE_REQUIRE(w && g && m && v && lr_t_dev && n > 0, "bad arguments");
   CAPE_REQUIRE(beta1 >= 0.f && beta1 < 1.f && beta2 >= 0.f && beta2 < 1.f && eps > 0.f, "bad Adam constants");
-  adam_kernel<<<blocks_for(n, 256, 148 * 8), 256, 0, (cudaStream_t)stream>>>(w, g, m, v, n, sumsq, clip_norm, lr_t_dev,
+  adam_kernel<<<blocks_for(n, 256, H100_SMS * 8), 256, 0, (cudaStream_t)stream>>>(w, g, m, v, n, sumsq, clip_norm, lr_t_dev,
                                                                               beta1, beta2, eps);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);

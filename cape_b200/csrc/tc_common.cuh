@@ -1,190 +1,77 @@
-// Device helpers shared by the tcgen05 / TMA kernels: mbarriers, proxy fences, UMMA issue, TMEM loads, TMA loads.
+// Device helpers shared by the wgmma kernels (sm_90a): shared-memory operand tiles, descriptors, wgmma fences, the
+// 3xTF32 operand split.
+//
+// Operand tiles are K-major with the 128-byte swizzle: one tile row holds 32 consecutive k (128 bytes), 16-byte chunk
+// j of row m sits at chunk j ^ (m & 7), rows follow each other every 128 bytes (8-row groups of 1024 bytes).  Tiles
+// start at 1024-byte boundaries, so a wgmma descriptor addresses the k-step ks (8 tf32 = 32 bytes) of a tile by adding
+// 32 * ks bytes to the start address.
 #pragma once
-#include <cuda.h>
 #include <stdint.h>
 #include "../../include/cape_b200.h"
+#include "wgmma_tf32.cuh"
 
 namespace cape {
 namespace tc {
 
-constexpr uint32_t SPIN_LIMIT = 1u << 27;   // trap instead of hanging the GPU if a barrier never flips
-
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+// wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B (layout type 1), stride between 8-row groups 1024 B
+__device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
+  return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+
+// byte offset of element (m, k) (k = 0..31) of a tile
+__device__ __forceinline__ uint32_t sw_off(int m, int k) {
+  return (uint32_t)(m * 128 + ((((k >> 2) ^ (m & 7)) << 4) | ((k & 3) << 2)));
 }
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t ok = 0, spins = 0;
-  while (true) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (ok) break;
-    if (++spins > SPIN_LIMIT) __trap();
-  }
-}
-// One leader lane of a fully converged warp.  The tcgen05 / TMA issue loops run on ALL 32 lanes (every value they compute
-// is warp-uniform, so it lives in uniform registers) and only the instruction itself sits under this predicate: issued
-// from an `if (lane == 0)` region instead, every UTCHMMA / UTMALDG is wrapped by the compiler in an ELECT / R2UR.BROADCAST /
-// BRA.U.ANY loop (~10 issue slots per MMA on the one thread the tensor pipe depends on).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(cols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(cols) : "memory");
-}
-// 16 accumulator columns of this thread's TMEM lane
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// keeps the compiler from moving accumulator reads or writes across the asynchronous MMAs
+template <int N>
+__device__ __forceinline__ void fence_acc(float (&d)[N]) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// same load without the wait: several can be in flight before one tmem_ld_wait()
-__device__ __forceinline__ void tmem_ld16_async(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+// 3xTF32 operand split: hi = x with the low 13 mantissa bits cleared (exactly representable in tf32), lo = x - hi
+__device__ __forceinline__ float tf32_hi(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 
-// 3xTF32 operand split of four values: hi = the top 19 bits (what the tensor core reads of a raw fp32 word), lo = x - hi;
-// both tiles get the value at the same byte offset
-__device__ __forceinline__ void split_store(float4 v, char* hi_tile, char* lo_tile, uint32_t off) {
+// four consecutive k of one tile row (16-byte aligned chunk) into the hi and lo tiles
+__device__ __forceinline__ void split_store4(float4 v, char* hi_tile, char* lo_tile, uint32_t off) {
   float4 h, l;
-  h.x = __uint_as_float(__float_as_uint(v.x) & 0xffffe000u); l.x = v.x - h.x;
-  h.y = __uint_as_float(__float_as_uint(v.y) & 0xffffe000u); l.y = v.y - h.y;
-  h.z = __uint_as_float(__float_as_uint(v.z) & 0xffffe000u); l.z = v.z - h.z;
-  h.w = __uint_as_float(__float_as_uint(v.w) & 0xffffe000u); l.w = v.w - h.w;
+  h.x = tf32_hi(v.x); l.x = v.x - h.x;
+  h.y = tf32_hi(v.y); l.y = v.y - h.y;
+  h.z = tf32_hi(v.z); l.z = v.z - h.z;
+  h.w = tf32_hi(v.w); l.w = v.w - h.w;
   *reinterpret_cast<float4*>(hi_tile + off) = h;
   *reinterpret_cast<float4*>(lo_tile + off) = l;
 }
-
-// Same with hi = the value ROUNDED to the nearest tf32 (low 13 bits zero, so the tensor core's truncation is a no-op):
-// lo = x - hi is then signed and at most half a tf32 ulp, the dropped lo*lo term and the truncation of lo are
-// zero-mean instead of a systematic shrink of every product.
-__device__ __forceinline__ float tf32_rn(float x) { return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u); }
-__device__ __forceinline__ void split_store_rn(float4 v, char* hi_tile, char* lo_tile, uint32_t off) {
-  float4 h, l;
-  h.x = tf32_rn(v.x); l.x = v.x - h.x;
-  h.y = tf32_rn(v.y); l.y = v.y - h.y;
-  h.z = tf32_rn(v.z); l.z = v.z - h.z;
-  h.w = tf32_rn(v.w); l.w = v.w - h.w;
-  *reinterpret_cast<float4*>(hi_tile + off) = h;
-  *reinterpret_cast<float4*>(lo_tile + off) = l;
+__device__ __forceinline__ void split_store1(float v, char* hi_tile, char* lo_tile, uint32_t off) {
+  const float h = tf32_hi(v);
+  *reinterpret_cast<float*>(hi_tile + off) = h;
+  *reinterpret_cast<float*>(lo_tile + off) = v - h;
 }
 
-// MN-major SWIZZLE_128B_BASE32B operand descriptor (layout_type 1), the only MN-major layout tcgen05 accepts for
-// 32-bit operands: 32-element MN blocks of 4096 B (LBO), 4-row K groups of 512 B (SBO), 128-byte rows whose 32-byte
-// chunks are XOR-ed with (row & 3)  [cute Layout_MN_SW128_32B_Atom, Swizzle<2,5,2>].  A TMA box of 32 floats x 32 rows
-// with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B writes exactly one such MN block.
-// LINEAR epilogue of 16 output columns of one row: bias (four 16-byte loads when the pointer allows it: a bias can be a
-// 4-byte-aligned view into a flat parameter buffer) and the activation, chosen once per call instead of per element.
-__device__ __forceinline__ void bias_act16(float (&v)[16], float (&o)[16], const float* bias, bool bias_vec, int act,
-                                           float alpha) {
-  if (bias != nullptr) {
-    if (bias_vec) {
+// acc += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo over one 32-deep chunk (four k-steps of 8), A = 64 rows of this warpgroup
+template <int N>
+__device__ __forceinline__ void mma3_chunk(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
+                                           uint32_t b_lo, int scale_first) {
 #pragma unroll
-      for (int j = 0; j < 16; j += 4) {
-        const float4 b4 = __ldg(reinterpret_cast<const float4*>(bias + j));
-        v[j] += b4.x; v[j + 1] += b4.y; v[j + 2] += b4.z; v[j + 3] += b4.w;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) v[j] += __ldg(bias + j);
-    }
-  }
-  if (act == CAPE_ACT_LEAKY) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) o[j] = v[j] > 0.f ? v[j] : alpha * v[j];
-  } else if (act == CAPE_ACT_RELU) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) o[j] = fmaxf(v[j], 0.f);
-  } else {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) o[j] = v[j];
+  for (int ks = 0; ks < 4; ++ks) {
+    const uint32_t adv = 32u * ks;
+    wg::mma_tf32<N>(d, make_desc(a_hi + adv), make_desc(b_hi + adv), ks == 0 ? scale_first : 1);
+    wg::mma_tf32<N>(d, make_desc(a_lo + adv), make_desc(b_hi + adv), 1);
+    wg::mma_tf32<N>(d, make_desc(a_hi + adv), make_desc(b_lo + adv), 1);
   }
 }
 
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3fffu) | ((uint64_t)(4096 >> 4) << 16) | ((uint64_t)(512 >> 4) << 32) |
-         (1ull << 46) | (1ull << 61);
-}
-
-// 2-D tiled TMA load: box at (c0 = innermost coordinate, c1) -> shared memory, completion on an mbarrier (tx bytes)
-__device__ __forceinline__ void tma_load_2d(uint32_t dst_smem, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
-      : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
-}
-
-// cuTensorMapEncodeTiled through the runtime's driver entry point table (no link-time dependency on libcuda);
-// nullptr if the driver does not provide it -- callers then keep their non-TMA path
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-inline EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  static bool tried = false;
-  if (!tried) {
-    tried = true;
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(ptr);
-    else
-      (void)cudaGetLastError();
-  }
-  return fn;
-}
+// accumulator fragment of m64nNk8 (f32): element i of thread `t` of the warpgroup is at
+//   row = 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),   col = 8 * (i / 4) + 2 * (t % 4) + (i % 2)
+__device__ __forceinline__ int frag_row(int t, int i) { return 16 * (t >> 5) + ((t & 31) >> 2) + 8 * ((i >> 1) & 1); }
+__device__ __forceinline__ int frag_col(int t, int i) { return 8 * (i >> 2) + 2 * (t & 3) + (i & 1); }
 
 }  // namespace tc
 }  // namespace cape

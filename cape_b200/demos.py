@@ -1,4 +1,4 @@
-"""`demo_simple`: the reference's clothing-generation demo (demos.py:339-406, run_simple_demo.py) on the B200 engine.
+"""`demo_simple`: the reference's clothing-generation demo (demos.py:339-406, run_simple_demo.py) on the H100 engine.
 
 Fix a body pose, run the four clothing types through the condition nets, draw latent codes, decode
 (`CAPE.decode`: decoder-only generation, the latency-sensitive serving path), de-normalise with the training-set

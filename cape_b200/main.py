@@ -1,5 +1,5 @@
 """`python -m cape_b200.main --config configs/<x>.yaml --mode train ...`: the reference's main.py (main.py:1-113) on
-the B200 engine.
+the H100 engine.
 
 Same flow: parse the config (the reference's yaml files load unchanged), load the dataset (`BodyData`), build the mesh
 hierarchy for `--num_conv_layers` / `--ds_factor`, construct `CAPE` and train.  The hierarchy is GENERATED from the

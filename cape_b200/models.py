@@ -1,4 +1,4 @@
-"""`CAPE`: the reference's model class (lib/models.py:230-1174) on top of the B200 kernels.
+"""`CAPE`: the reference's model class (lib/models.py:230-1174) on top of the H100 kernels.
 
 Same constructor keywords as `models.CAPE(L=, D=, U=, L_d=, D_d=, **params)` built by main.py:50-87, same
 public methods (`build_graph`, `fit`, `encode`, `encode_only_condition`, `predict`, `evaluate`, `decode`,

@@ -44,7 +44,7 @@ class ParamStore:
         self.flat = torch.zeros(self.size, device=device)
         self.grad = torch.zeros(self.size, device=device)
         self.mom = torch.zeros(self.size, device=device)
-        self.lo = torch.zeros(self.size, device=device)     # flat - tf32_trunc(flat): weight tiles by TMA (3xTF32)
+        self.lo = torch.zeros(self.size, device=device)     # flat - tf32_trunc(flat): cape_term.wT_lo (unread by the wgmma kernels)
         self.var = None                                     # Adam's second-moment slot (`mom` is its first): add_adam_slot()
 
     def add_adam_slot(self):
@@ -106,7 +106,7 @@ class Arena:
 def choose_dw_mode(F, Fout, K, rows_in, rows_out, need_dx, stash=True):
     """Where a layer's weight gradient takes its operands from (see ChebLayer): "aside" = basis stashed by the forward
     kernel, "gside" = op^T G stashed by the data-gradient kernel, "gather" = gathered again by cape_cheb_dw.
-    The dense TMA kernel needs F % 4 == 0, F >= 32 and 32 | Fout <= 512; pooled sites contract over the (fewer)
+    The dense weight-gradient kernel needs F % 4 == 0, F >= 32 and 32 | Fout <= 512; pooled sites contract over the (fewer)
     output rows, un-pooling ones over the (fewer) input rows, same-level ones take the narrower side."""
     dense_ok = F % 4 == 0 and F >= 32 and Fout % 32 == 0 and Fout <= 512
     if not (dense_ok and stash):
@@ -118,20 +118,21 @@ def choose_dw_mode(F, Fout, K, rows_in, rows_out, need_dx, stash=True):
     return "aside"
 
 
-def choose_forms(F, C, Fout, K, rows_in, rows_out, affine, need_dx, dw_mode, precise, plain, name="", env=None):
+def choose_forms(F, C, Fout, K, rows_in, rows_out, affine, need_dx, dw_mode, plain, name="", env=None):
     """(fwd_mode, dx_mode) of a conv layer -- how its forward / data-gradient pass is organised (the math is the same):
       "fused":    one kernel gathers the basis and contracts it (ellconv_tc.cu; thin layers: thin.cu);
       "basis":    cape_apply writes B_k = op_k x (forward: the stash the weight gradient reads anyway) or H_k = op_k^T G
-                  (data gradient), then the TMA-fed kernel contracts plain tensors;
-      "contract": the TMA-fed kernel computes Z = x @ [W_0 | W_1 | ..] (or G @ [W_k^T]_k) on the SOURCE rows, then
+                  (data gradient), then the tensor-core kernel contracts plain tensors;
+      "contract": the tensor-core kernel computes Z = x @ [W_0 | W_1 | ..] (or G @ [W_k^T]_k) on the SOURCE rows, then
                   cape_apply applies the operators to the narrower Z and runs the epilogue.
-    Defaults from the per-layer measurements at batch 64 (profiles/r02_launch_profile.csv):
-      * forward: basis-first where the short-chain accumulation is wanted (it needs plain operands: the encoder) and for
-        the pooled K = 3 discriminator layers, contract-first for un-pooling layers (half the rows in the contraction, Fout-wide gathers: dec/aff3 420 -> 265 us)
-        and for precise decoder blocks, fused elsewhere (discriminator: three gathers + a contraction lose to one kernel);
+    The defaults follow the work each form does; they have not been re-measured per layer on the H100:
+      * forward: basis-first for the pooled K = 3 discriminator layers (the composed T_2 operator has ~19 taps, and the
+        gathered basis is the stash the weight gradient reads anyway), contract-first for un-pooling layers (half the
+        rows in the contraction, Fout-wide gathers), fused elsewhere;
       * data gradient: contract-first when the gradient narrows (Fout > F: the gathers run on the narrow side) or the
-        layer pools and is at least 128 wide (the contraction runs on half the rows: disc/conv3 495 -> 333 us);
-        basis-first only for the wide un-pooling block (every other decoder layer is faster fused).
+        layer pools and is at least 128 wide (the contraction runs on half the rows); basis-first for the wide
+        un-pooling block only.
+    Every tensor-core contraction accumulates in short per-chunk chains, so accuracy does not pick a form.
     Experiment overrides: CAPE_FWD_MODE / CAPE_DX_MODE for every layer, CAPE_MODES="enc/conv8:fwd=fused,disc/conv3:dx=contract"
     for single ones (ineligible requests are ignored).  `plain`: every operator of the site is the identity."""
     env = os.environ if env is None else env
@@ -140,14 +141,11 @@ def choose_forms(F, C, Fout, K, rows_in, rows_out, affine, need_dx, dw_mode, pre
     fwd_mode, dx_mode = "fused", "fused"
     basis_ok = C == 0 and not affine and dw_mode == "aside"
     if split_ok:
-        if precise and basis_ok:
-            fwd_mode = "basis"
-        elif basis_ok and K >= 3 and rows_out < rows_in:
+        if basis_ok and K >= 3 and rows_out < rows_in:
             # pooled K = 3 layers (the discriminator): the composed T_2 operator has ~19 taps, and the stash the fused kernel
-            # writes next to its gather is what the separate gather launch produces anyway (round-2b per-layer profile:
-            # disc/conv4 189 -> 136 us, conv2 273 -> 261, conv3 unchanged)
+            # writes next to its gather is what the separate gather launch produces anyway
             fwd_mode = "basis"
-        elif (C > 0 or affine) and (rows_in < rows_out or precise):
+        elif (C > 0 or affine) and rows_in < rows_out:
             fwd_mode = "contract"
         # (an affine block has TWO upstream gradients -- d out and d out masked by the ReLU branch -- and the contract-first
         # data gradient projects only one tensor: fused for those.  No shipped config has an affine block that widens,
@@ -157,8 +155,7 @@ def choose_forms(F, C, Fout, K, rows_in, rows_out, affine, need_dx, dw_mode, pre
             dx_mode = "contract"
         if need_dx and dw_mode == "gside" and rows_in < rows_out and Fout >= 128:
             # wide un-pooling block (dec/aff3: 256 -> 128 at 862 -> 1723 rows): H = op^T G by the gather kernel into the
-            # weight gradient's stash, then one plain contraction -- 290 -> 245 us; the narrower un-pooling blocks (aff5,
-            # aff7) lose 15-20 % that way and stay fused
+            # weight gradient's stash, then one plain contraction; the narrower un-pooling blocks stay fused
             dx_mode = "basis"
     fm, dm = env.get("CAPE_FWD_MODE", ""), env.get("CAPE_DX_MODE", "")
     for item in filter(None, env.get("CAPE_MODES", "").split(",")):
@@ -180,7 +177,7 @@ class ChebLayer:
     branch) with its backward."""
 
     def __init__(self, net, site, F, C, Fout, W, gW, bias=None, gbias=None, act=ACT_NONE, Wa=None, gWa=None,
-                 bias_per_row=False, need_dx=True, maxN=1, n_cs_slots=1, name="", precise=False):
+                 bias_per_row=False, need_dx=True, maxN=1, n_cs_slots=1, name=""):
         self.net, self.tp, self.site, self.name = net, net.tp, site, name
         if (bias is not None or act != ACT_NONE) and not site.pool_is_selection:
             raise NotImplementedError("%s: the down-sampling matrix is not a pure row selection, so pooling cannot be "
@@ -195,7 +192,6 @@ class ChebLayer:
         if self.affine:
             self.Wa, self.Wa2, self.gWa2 = Wa, Wa.view(F + C, Fout), gWa.view(F + C, Fout)
         self.need_dx = need_dx
-        self.precise = bool(precise)
         dev = W.device
         # Derived weight layouts, refreshed after every update by ONE batched launch (net.wprep):
         #   Wt [K(+1), Fout, F]: per-order K-major copies (+ the affine branch as order K): B operand of the tensor-core
@@ -212,9 +208,9 @@ class ChebLayer:
         # Where the weight gradient gets its operands (all three end in the same contraction  dW = A^T G over rows):
         #   "aside":  the forward kernel also writes the gathered basis B_k = op_k x (cape_term.stash), dW_k = B_k^T G;
         #   "gside":  the data-gradient kernel also writes H_k = op_k^T G, dW_k = x^T H_k -- all K terms in ONE pass
-        #             over x when K*Fout <= 512 (the TMEM width), over the smaller row set when the site un-pools;
+        #             over x when K*Fout <= 512 (the widest weight-gradient tile set), over the smaller row set when the site un-pools;
         #   "gather": cape_cheb_dw gathers the basis again (thin layers, odd shapes).
-        # The first two make both operands plain tensors, which is what the TMA-fed tcgen05 kernel wants.
+        # The first two make both operands plain tensors, which the weight-gradient kernel reads without a gather.
         self.dw_mode = choose_dw_mode(F, Fout, K, site.rows_in, site.rows_out, need_dx,
                                       os.environ.get("CAPE_DW_STASH", "1") != "0")
         self.stash_a, self.stash_g, self.stash_ga = [None] * K, [None] * K, None
@@ -236,7 +232,7 @@ class ChebLayer:
             if self.affine and site.opsT[0] != -1:
                 self.stash_ga = torch.empty(maxN, site.rows_in, Fout, device=dev)
         self.fwd_mode, self.dx_mode = choose_forms(F, C, Fout, K, site.rows_in, site.rows_out, self.affine, need_dx,
-                                                   self.dw_mode, self.precise, all(o == -1 for o in site.ops), name)
+                                                   self.dw_mode, all(o == -1 for o in site.ops), name)
         if self.dx_mode == "contract":
             self.Wk, self.Wk_lo = torch.empty(K, F, Fout, device=dev), torch.empty(K, F, Fout, device=dev)
             net.wprep.add(W, F, K, Fout, wk=self.Wk, wk_lo=self.Wk_lo)
@@ -292,7 +288,7 @@ class ChebLayer:
             cheb_call(self.tp, N, s.rows_in, ncz,
                       [dict(src=x, op=-1, F=F, src_rows=s.rows_in, src_stride=sx, w=None, w_stride=0,
                             wT=self.Wt.view(ncz, F), wT_stride=F, wT_lo=self.Wt_lo.view(ncz, F))],
-                      Z, plain_only=True, precise=self.precise, tag=sub("project"))
+                      Z, plain_only=True, tag=sub("project"))
             terms = [dict(src=Z[:, :, k * Fout:], op=s.ops[k], src_rows=s.rows_in, src_stride=ncz, acc=0,
                           wc=self.W3[F:, k, :] if C else None, wc_stride=K * Fout) for k in range(K)]
             if self.affine:
@@ -331,7 +327,7 @@ class ChebLayer:
             terms.append(t)
         cheb_call(self.tp, N, s.rows_out, Fout, terms, out, out2=out2, cond=ycat if C else None,
                   epilogue=EPI_AFFINE if self.affine else EPI_LINEAR, act=self.act, bias=self.bias,
-                  bias_per_row=self.bias_per_row, tag=tag, precise=self.precise)
+                  bias_per_row=self.bias_per_row, tag=tag)
 
     def bwd(self, x, ycat, g, g_aff=None, dx=None, dx2=None, dx_epi=EPI_LINEAR, dx_aux=None, dx_alpha=E.LEAKY_ALPHA,
             dycat=None, want_dw=True, cs_slot=0):
@@ -596,9 +592,8 @@ class CapeNetwork:
         """reorder: keep the hidden activations in patch order (topology.patch_order) instead of the reference's
         vertex numbering.  Everything visible from outside (inputs, outputs, parameters, their gradients, the
         FC-layer row layout) stays in the reference numbering: the permutations are folded into the operator
-        tables of the first/last conv of each stack.  Default: off (env CAPE_REORDER=1 turns it on): measured
-        neutral on B200 (4066 vs 4069 meshes/s) -- a gather batch waits for its slowest load whatever the L1 hit
-        rate; kept because the shared-memory halo staging planned next needs compact tiles."""
+        tables of the first/last conv of each stack.  Default: off (env CAPE_REORDER=1 turns it on): a gather batch
+        waits for its slowest load whatever the L1 hit rate; kept because the shared-memory halo staging planned next needs compact tiles."""
         self.cfg = dict(cfg)
         if reorder is None:
             reorder = os.environ.get("CAPE_REORDER", "0") == "1"
@@ -626,7 +621,7 @@ class CapeNetwork:
         self.dw_stream = torch.cuda.Stream(device=dev) if self.async_dw else None
         self._dw_pending = False
         # column sums (bias / condition-channel gradients) off the main stream, their small products in ONE launch at the
-        # end of the backward pass (CAPE_SIDE_GLUE=0: in line, one launch per player -- the round-2a schedule)
+        # end of the backward pass (CAPE_SIDE_GLUE=0: in line, one launch per player)
         self.side_glue = self.async_dw and os.environ.get("CAPE_SIDE_GLUE", "1") != "0"
         self.p = [int(l.shape[0]) for l in L]
         self.p_d = [int(l.shape[0]) for l in L_d]
@@ -659,13 +654,6 @@ class CapeNetwork:
         else:
             og, od = [None] * (nl + 1), [None] * (len(D_d) + 1)
         self.order_g, self.order_d = og, od
-        # The encoder's forward convs keep their tensor-core accumulation chains short (cape_conv_args.precise): their
-        # rounding error is what exp(logvar) amplifies (sigma = exp(logvar / 2) reaches 1e2 with the reference's
-        # initialisers); everywhere else the plain 3xTF32 accumulation is well inside the 1e-4 gate.
-        precise_enc = os.environ.get("CAPE_PRECISE_ENCODER", "1") != "0"
-        # the first decoder blocks have the longest reductions after the encoder (576 and 320 channels x K): the number
-        # of leading blocks that run contract-first with the short-chain projection (x_hat accuracy, not amplified)
-        precise_dec = int(os.environ.get("CAPE_PRECISE_DECODER", "0"))
         self.enc = []
         fin = c["nn_input_channel"]
         for i in range(nl):
@@ -673,13 +661,13 @@ class CapeNetwork:
             sc = "generator/encoder/encoder_conv%d" % (i + 1)
             self.enc.append(ChebLayer(self, site, fin, 0, F[i], w(sc + "/weights"), g(sc + "/weights"),
                                       bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=ACT_LEAKY, need_dx=(i > 0),
-                                      maxN=N, name="enc/conv%d" % (i + 1), precise=precise_enc))
+                                      maxN=N, name="enc/conv%d" % (i + 1)))
             fin = F[i]
         red = specs["generator/encoder/1x1-conv/weights"][1]
         self.red = red
         self.enc_1x1 = ChebLayer(self, ConvSite(tp, L[-1], 1, order_in=og[nl]), F[-1], 0, red,
                                  w("generator/encoder/1x1-conv/weights"),
-                                 g("generator/encoder/1x1-conv/weights"), maxN=N, name="enc/1x1", precise=precise_enc)
+                                 g("generator/encoder/1x1-conv/weights"), maxN=N, name="enc/1x1")
         flat = self.p[-1] * red
         self.flat = flat
         dn = lambda s, act=ACT_NONE: Dense(self, w(s + "/dense/kernel").view(specs[s + "/dense/kernel"]),
@@ -700,8 +688,7 @@ class CapeNetwork:
                 sc = "generator/decoder/decoder_resblock_affine%d" % (i + 1)
                 self.dec.append(ChebLayer(self, site, fin, Cc, Fo, w(sc + "/graph_conv/weights"),
                                           g(sc + "/graph_conv/weights"), Wa=w(sc + "/affine/weights"),
-                                          gWa=g(sc + "/affine/weights"), maxN=N, name="dec/aff%d" % (i + 1),
-                                          precise=i < precise_dec))
+                                          gWa=g(sc + "/affine/weights"), maxN=N, name="dec/aff%d" % (i + 1)))
             else:
                 Fo = F[-i - 1]
                 self.dec.append(GNBlock(self, i, L[-i - 2], U[-i - 1], fin, Cc, Fo, K[-i - 1],
@@ -1136,7 +1123,7 @@ class CapeNetwork:
         buffer is all-reduced in three buckets as soon as each is final -- decoder (+ the discriminator's buffer) after
         the decoder backward, the two 28 MB encoder FC kernels right after their weight gradients, the encoder convs /
         condition nets at the end -- on a communication stream that the backward pass does not wait for until its very
-        end.  Verified eagerly on two B200s (replicas bit-identical, gradients of the global batch); captured inside the
+        end.  Checked eagerly on two GPUs (replicas bit-identical, gradients of the global batch); captured inside the
         forward/backward graph the step also completes, but destroying the process group afterwards hung in the one
         run the budget allowed, so `bench.py` and `CAPE.fit` keep the default.  world <= 1 switches it off."""
         if world <= 1:

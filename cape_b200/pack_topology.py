@@ -1,19 +1,21 @@
 #!/usr/bin/env python
-"""Converter: the reference checkout's operator fixtures -> one pickle-free .npz next to this package.
+"""Converter: the reference checkout's operator fixtures -> pickle-free .npz fixtures under tests/golden/.
 
 The reference ships its fixed mesh hierarchy as pickled scipy CSC matrices
 (<CAPE checkout>/data/transform_matrices/{for_demo,ds2}/{A,D,U}.npy, loaded at lib/load_data.py:7-32 with
-encoding='latin1').  Those files are covered by the reference's licence (no redistribution), so this repository
-does NOT contain them or anything derived loss-free from them: the .npz is generated locally from the user's own
-checkout of qianlim/CAPE and is git-ignored.  It holds the operators as plain CSR arrays
+encoding='latin1').  Those files are the fixed SMPL mesh hierarchy every model of CAPE runs on, so the
+repository keeps this converted copy as test data (tests/golden/smpl_topology_{for_demo,ds2,assets}.npz, split to keep
+each file small); the package loads its hierarchy from there.  Licence: the files are derived from data the reference
+distributes under its own licence (its LICENSE file: no redistribution; the template mesh and edge table are SMPL data
+under the SMPL licence).  They are kept here as test fixtures of that data; whoever redistributes this repository must
+have the right to redistribute them.
+It holds the operators as plain CSR arrays
 (indptr/indices/data/shape), the SMPL edge table (data/edges_smpl.npy, used by lib/losses.py:9-25; = upper triangle
 of A[0], checked against the reference file), the per-vertex normalisation statistics
 (data/demo_data/trainset_stats.npz, demos.py:155), the clothing-vertex index list, the template mesh and the demo
 poses (demos.py:349-357).
 
-    python -m cape_b200.pack_topology [--reference /path/to/CAPE]        (default: $CAPE_REFERENCE, /root/reference)
-
-`__graft_entry__.build()` runs it when the file is missing; `cape_b200.topology` does so on first use.
+    python -m cape_b200.pack_topology --reference /path/to/CAPE        (default: $CAPE_REFERENCE)
 """
 import argparse
 import os
@@ -21,14 +23,15 @@ import sys
 import numpy as np
 import scipy.sparse as sp
 
-OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data", "smpl_topology.npz")
+OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden")
+PARTS = ("for_demo", "ds2", "assets")     # one file per hierarchy; the edge table, statistics and demo assets
 
 
 def default_reference():
-    """The reference checkout to read the fixtures from: $CAPE_REFERENCE, else /root/reference; None if absent."""
-    for cand in (os.environ.get("CAPE_REFERENCE"), "/root/reference"):
-        if cand and os.path.isdir(os.path.join(cand, "data", "transform_matrices")):
-            return cand
+    """The reference checkout to read the fixtures from: $CAPE_REFERENCE; None if unset or absent."""
+    cand = os.environ.get("CAPE_REFERENCE")
+    if cand and os.path.isdir(os.path.join(cand, "data", "transform_matrices")):
+        return cand
     return None
 
 
@@ -72,22 +75,22 @@ def pack(REF, OUT=OUT):
     out["template.v"], out["template.f"] = np.asarray(v, np.float64), np.asarray(f, np.int32)
     dp = np.load(os.path.join(REF, "data", "demo_data", "demo_pose_params.npz"))
     out["demo.rot"], out["demo.pose"] = dp["rot"], dp["pose"]
-    os.makedirs(os.path.dirname(OUT), exist_ok=True)
-    tmp = OUT + ".tmp.%d.npz" % os.getpid()
-    np.savez_compressed(tmp, **out)
-    os.replace(tmp, OUT)                     # atomic: concurrent ranks may all find the file missing
+    os.makedirs(OUT, exist_ok=True)
+    for name in PARTS:
+        keys = [k for k in out if k.split(".")[0] == name or (name == "assets" and k.split(".")[0] not in PARTS)]
+        np.savez_compressed(os.path.join(OUT, "smpl_topology_%s.npz" % name), **{k: out[k] for k in keys})
     return OUT
 
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--reference", default=default_reference(), help="checkout of qianlim/CAPE")
-    ap.add_argument("--out", default=OUT)
+    ap.add_argument("--out", default=OUT, help="directory of the two .npz files")
     a = ap.parse_args(argv)
     if not a.reference:
         ap.error("no reference checkout found: pass --reference or set CAPE_REFERENCE")
     out = pack(a.reference, a.out)
-    print("wrote", os.path.abspath(out), os.path.getsize(out), "bytes")
+    print("wrote smpl_topology_{%s}.npz to %s" % (",".join(PARTS), os.path.abspath(out)))
 
 
 if __name__ == "__main__":

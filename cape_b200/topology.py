@@ -3,8 +3,8 @@
 Host-side counterpart of the reference's topology prep:
   - `laplacian`, `rescale_L`  : lib/mesh_sampling.py:10-38 (same names, same arithmetic in fp32)
   - `load_graph_mtx`          : lib/load_data.py:7-32 (same return convention) -- reads the pickle-free
-                                copy of data/transform_matrices/** that cape_b200/pack_topology.py makes
-                                from the user's reference checkout (licensed data: not part of this repo)
+                                copy of data/transform_matrices/** that cape_b200/pack_topology.py made
+                                (tests/golden/smpl_topology_*.npz)
 The reference turns every scipy matrix into a tf.SparseTensor and runs one SpMM per Chebyshev order and
 per pool/unpool (lib/models.py:74-96,141-149).  Here the operators are constants, so they are composed
 offline:  op_k = D . T_k(L~) . U  -- one sparse "row-gather" per polynomial order with pooling (row
@@ -15,7 +15,8 @@ import os
 import numpy as np
 import scipy.sparse as sp
 
-_DATA = os.path.join(os.path.dirname(os.path.abspath(__file__)), "data", "smpl_topology.npz")
+_DATA = [os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
+                      "smpl_topology_%s.npz" % part) for part in ("for_demo", "ds2", "assets")]
 _cache = {}
 
 
@@ -43,16 +44,11 @@ def rescale_L(L, lmax=2):
 
 def _npz():
     if "npz" not in _cache:
-        if not os.path.exists(_DATA):
-            from . import pack_topology
-            ref = pack_topology.default_reference()
-            if ref is None:
-                raise FileNotFoundError(
-                    "%s missing and no reference checkout to build it from: the SMPL mesh hierarchy is licensed data of "
-                    "qianlim/CAPE and is not shipped here.  Run `python -m cape_b200.pack_topology --reference "
-                    "/path/to/CAPE` (or set CAPE_REFERENCE) once." % _DATA)
-            pack_topology.pack(ref, _DATA)
-        _cache["npz"] = np.load(_DATA)
+        z = {}
+        for path in _DATA:
+            with np.load(path) as f:
+                z.update({k: f[k] for k in f.files})
+        _cache["npz"] = z
     return _cache["npz"]
 
 
@@ -97,16 +93,12 @@ def clothing_verts_idx():
 def template_mesh():
     """(vertices [6890, 3] float64, faces [13776, 3] int32) of data/template_mesh.obj (demos.py:352-353)."""
     z = _npz()
-    if "template.v" not in z.files:
-        raise FileNotFoundError("%s predates the demo assets: delete it and re-run cape_b200.pack_topology" % _DATA)
     return z["template.v"], z["template.f"]
 
 
 def demo_pose_params():
     """(rot [6, 216], pose [6, 72]) of data/demo_data/demo_pose_params.npz (demos.py:355-356)."""
     z = _npz()
-    if "demo.rot" not in z.files:
-        raise FileNotFoundError("%s predates the demo assets: delete it and re-run cape_b200.pack_topology" % _DATA)
     return z["demo.rot"], z["demo.pose"]
 
 

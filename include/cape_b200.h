@@ -1,5 +1,5 @@
 /*
- * cape_b200.h -- C ABI of libcape_b200.so: the B200 (sm_100a) implementation of CAPE's graph-conv hot path.
+ * cape_b200.h -- C ABI of libcape_b200.so: the H100 (sm_90a) implementation of CAPE's graph-conv hot path.
  *
  * The reference (qianlim/CAPE, TF-1.13) has no FFI; its operator seam is name-based dispatch on
  * `base_model` (lib/models.py:16-17,58-62: filter='chebyshev5', pool/unpool='poolwT',
@@ -71,20 +71,20 @@ typedef struct {
   const float* wc;    /* condition rows for accumulator 0 (NULL: none) */
   const float* wc2;   /* condition rows for accumulator 1 (NULL: none) */
   /* optional K-major copies of w / w2 (element (f, c) = wT[c * wT_stride + f]); when given for every term and the
-   * shapes allow it the contraction runs on the tcgen05 tensor cores (3xTF32, fp32-accurate), else on the fp32 pipe */
+   * shapes allow it the contraction runs on the wgmma tensor cores (3xTF32, fp32-accurate), else on the fp32 pipe */
   const float* wT;
   const float* w2T;
   int wT_stride;
   int w2T_stride;
   /* optional: also write this term's gathered basis rows  B[n, r, 0:F] = sum_j op[r, j] * src[n, idx[r, j], 0:F]  to
    * stash[(n * rows_out + r) * stash_stride + f]  (16-byte aligned, stash_stride % 4 == 0, F % 4 == 0).  The weight
-   * gradient of the layer can then contract plain tensors (cape_cheb_dw with op = -1: the TMA-fed kernel) instead of
+   * gradient of the layer can then contract plain tensors (cape_cheb_dw with op = -1: the dense-operand kernel) instead of
    * gathering again: in a forward call the stash is the basis itself, in a data-gradient call it is op^T . G, the
    * "narrow side" operand (dW_k = x^T (op_k^T G)). */
   float* stash;
   int stash_stride;
   /* optional: low parts of wT / w2T (x - tf32_trunc(x), same layout; cape_tf32_lo or cape_cheb_weight_transpose
-   * make them).  With them the wide-output kernel fetches its weight tiles by TMA (raw fp32 tile = "hi" operand). */
+   * make them).  Accepted for compatibility; the wgmma kernels split the weights on chip and do not read them. */
   const float* wT_lo;
   const float* w2T_lo;
 } cape_term;
@@ -111,12 +111,10 @@ typedef struct {
   const float* aux;    /* [N, rows_out, ncols] (SLOPE / DUALMASK) */
   float* out;          /* [N, rows_out, ncols] */
   float* out2;         /* [N, rows_out, ncols] or NULL */
-  /* 1: keep the tensor-core accumulation chains short (several TMEM accumulators per output, summed in fp32 by the
-   * epilogue).  The tcgen05 accumulator truncates on every accumulate, which shrinks long dot products by ~2^-25 per
-   * MMA; the encoder's forward convs ask for this because the VAE's exp(logvar) amplifies their error.  Honoured by the
-   * plain-operand (all terms identity) LINEAR-epilogue path; ignored elsewhere. */
+  /* Accepted for compatibility and without effect: every tensor-core contraction keeps its accumulation chains short
+   * (a fresh accumulator per 32-deep chunk, summed in fp32 with round-to-nearest), which is what 1 used to ask for. */
   int precise;
-  /* 1: fail (rc < 0) instead of falling back to the gather / fp32-pipe kernels when the TMA-fed plain-operand kernel
+  /* 1: fail (rc < 0) instead of falling back to the gather / fp32-pipe kernels when the plain-operand tensor-core kernel
    * cannot take the call -- for callers that only filled wT / wT_lo (the `w` pointers are then never read). */
   int plain_only;
 } cape_conv_args;
@@ -125,7 +123,7 @@ typedef struct {
  *   acc_a[n, r, c] = sum_{t: acc_t = a} scale_t * ( sum_j op_t[r, j] * src_t[n, idx_t[r, j], c]
  *                                                   + rowsum(op_t)[r] * (cond[n, :C] @ wc_t[:C, c]) ),     c < ncols
  * then the epilogue of cape_conv_args (LINEAR: bias + activation; AFFINE: out = acc1 + relu(acc0), out2 = relu(acc0);
- * SLOPE / DUALMASK with aux).  With the TMA-fed contraction of plain tensors (cape_cheb_fwd, all terms identity) this
+ * SLOPE / DUALMASK with aux).  With the tensor-core contraction of plain tensors (cape_cheb_fwd, all terms identity) this
  * gives the two split forms of chebyshev5 (+poolwT, +fit_cond_dim; lib/models.py:69-103,129-152,813-832):
  *   contract first:  Z = X @ [W_0 | W_1 | ...]   (cape_cheb_fwd),   out = epi(sum_k op_k Z_k)   (cape_apply)
  *   basis first:     B_k = op_k X                 (cape_apply),      out = epi(sum_k B_k W_k)    (cape_cheb_fwd)
@@ -162,16 +160,12 @@ typedef struct {
 int cape_apply(cape_topology* t, const cape_apply_args* a, void* stream);
 
 /* Experiment knobs (process-wide, 16 integer slots, all 0 by default = the shipped configuration).  They switch single
- * optimisations off for A/B measurements and fallback-path tests: [1]=1 no TMA dense weight-gradient kernel, [3]=2
- * 128- instead of 256-wide column sub-tiles in it, [4]=1 conv weight tiles by the producer warps instead of TMA,
- * [5]=1 one narrow-conv CTA per SM, [6]=1 identity-term basis tiles by the producer warps, [7]=1 thin-output layers
- * on the generic kernels, [8]=1 no TMA-fed plain-operand conv kernel, [9]=1 no reduction-order rotation in it,
- * [10]=rows per CTA of cape_apply (16..1024), [15]=1 the plain-operand kernel derives its weight lo tiles on chip
- * instead of fetching them from cape_term.wT_lo, [11..14]=its ring depths then (A lo, weight lo, A raw, weight raw) ([0] and [2] are diagnostics
- * of the operand split).  Returns the previous value, <0 for an unknown key. */
+ * optimisations off for A/B measurements and fallback-path tests: [7]=1 thin-output layers on the generic kernels,
+ * [8]=1 no tensor-core plain-operand conv path, [10]=rows per CTA of cape_apply (16..1024), [16]=1 scalar FC kernel,
+ * [17]=1 fixed CTA count of the thin weight gradient.  Returns the previous value, <0 for an unknown key. */
 int cape_set_tuning(int key, int value);
 
-/* Process-wide switch for the tcgen05 path of cape_cheb_fwd (default on); returns the previous setting. */
+/* Process-wide switch for the tensor-core path of cape_cheb_fwd (default on); returns the previous setting. */
 int cape_set_tensor_cores(int enable);
 int cape_tensor_cores_enabled(void);
 

@@ -1,5 +1,16 @@
 """Seeded inputs of the golden op cases (shared by make_golden.py and the tests; outputs are committed)."""
+import hashlib
+
 import numpy as np
+
+# ops_golden.npz keeps every OPS_VSTRIDE-th vertex of each output (the file stays under 1 MB)
+OPS_VSTRIDE = 4
+
+
+def digest(a):
+    """SHA-256 of an array's dtype, shape and bytes: what lap_golden.npz stores for a bit-for-bit comparison."""
+    a = np.ascontiguousarray(a)
+    return hashlib.sha256(("%s%s" % (a.dtype.str, a.shape)).encode() + a.tobytes()).hexdigest()
 
 
 def golden_inputs():

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Golden vectors from the REFERENCE's own model code.  Runs only where /root/reference (or $CAPE_REFERENCE) exists.
+"""Golden vectors from the REFERENCE's own model code.  Runs only where $CAPE_REFERENCE names a checkout.
 
 `lib/models.py` of the reference is imported UNMODIFIED and executed on the TensorFlow-1 API shim of
 oracle/tf1_shim.py (torch-CPU behind the ~70 TF symbols the file calls): `CAPE.build_graph(phase='train')` then runs
@@ -31,7 +31,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.abspath(os.path.join(HERE, "..", ".."))
-REF = os.environ.get("CAPE_REFERENCE", "/root/reference")
+REF = os.environ.get("CAPE_REFERENCE", "")
 for p in (ROOT, os.path.join(ROOT, "tests")):
     if p not in sys.path:
         sys.path.insert(0, p)
@@ -39,6 +39,23 @@ if REF not in sys.path:
     sys.path.append(REF)            # last: only `lib` (the reference's package) is meant to resolve there
 
 OUT = os.path.join(HERE, "ref_models_golden.npz")
+# the arrays are stored in two files of under 1 MB each, split by the first component of their key
+PARTS = {"ref_models_golden.npz": ("nz64", "nz64_l4", "ops"), "ref_models_golden_2.npz": ("nz18", "nz64_u2")}
+
+
+class Golden(dict):
+    """The golden arrays of both files, read like one np.load result (`z[key]`, `z.files`)."""
+    @property
+    def files(self):
+        return list(self)
+
+
+def load():
+    z = Golden()
+    for name in PARTS:
+        with np.load(os.path.join(HERE, name)) as f:
+            z.update({k: f[k] for k in f.files})
+    return z
 NSAMPLE = 64
 OPS_STRIDE = 8
 
@@ -242,8 +259,9 @@ def main():
         store["ops/" + k] = v.astype(np.float32).reshape(-1)[::OPS_STRIDE]         # every 8th element keeps the file small
         print("ops %s: reference vs the committed known answer (numpy transcription): max rel %.2e"
               % (k, np.abs(v - prev[k]).max() / np.abs(prev[k]).max()))
-    np.savez_compressed(OUT, **store)
-    print("wrote", OUT, os.path.getsize(OUT), "bytes")
+    for name, heads in PARTS.items():
+        np.savez_compressed(os.path.join(HERE, name), **{k: v for k, v in store.items() if k.split("/")[0] in heads})
+        print("wrote", name, os.path.getsize(os.path.join(HERE, name)), "bytes")
 
 
 if __name__ == "__main__":

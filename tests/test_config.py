@@ -1,11 +1,15 @@
 """parse_config: reference flags/defaults/precedence; the reference's own yaml files load unchanged."""
 import os
+import sys
 
+import numpy as np
 import pytest
 
 from cape_b200.config_parser import model_params, parse_config
 
-REF_CFG = "/root/reference/configs"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
+sys.path.insert(0, GOLDEN)
+import make_host_golden as H  # noqa: E402
 
 AFFINE_YAML = """dataset: dataset_male_4clotypes
 name: CAPE-affineconv_nz64_pose32_clotype32_male
@@ -56,10 +60,15 @@ def test_defaults_without_file(tmp_path, monkeypatch):
         parse_config(["--config", "missing.yaml"])
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_CFG), reason="reference tree not present (GPU box)")
-def test_reference_configs_load_unchanged():
-    for fn in sorted(os.listdir(REF_CFG)):
-        args, _ = parse_config(["--config", os.path.join(REF_CFG, fn)])
+def test_reference_configs_load_unchanged(tmp_path):
+    """The reference's own configs/*.yaml (their text is kept in tests/golden/ref_configs.npz) parse unchanged."""
+    z = np.load(H.CONFIGS_OUT)
+    names = z["names"].tolist()
+    assert any(n.startswith("CAPE-affineconv_nz64") for n in names) and any(n.startswith("CAPE_nz18") for n in names)
+    for fn, text in zip(names, z["texts"].tolist()):
+        path = tmp_path / fn
+        path.write_text(text)
+        args, _ = parse_config(["--config", str(path)])
         if fn.startswith("CAPE-affineconv_nz64"):
             assert (args.nz, args.nz_cond, args.nz_cond2, args.affine) == (64, 32, 32, 1)
         if fn.startswith("CAPE_nz18"):
@@ -101,74 +110,53 @@ def test_layer_forms_of_the_shipped_config():
     """choose_forms (fused / basis-first / contract-first) on the nz64 layer shapes, and its overrides."""
     from cape_b200.network import choose_forms as f
     env = {}
-    # encoder conv2 (pooled 64 -> 64, precise): basis-first forward; the data gradient stays fused (64 wide)
-    assert f(64, 0, 64, 2, 6890, 3445, False, True, "aside", True, False, "enc/conv2", env) == ("basis", "fused")
-    # encoder conv3 (64 -> 128): the gradient narrows -> contract first; conv6 (pooled, 256 wide) too; conv8 (K*F > 512) not
-    assert f(64, 0, 128, 2, 3445, 3445, False, True, "aside", True, False, "enc/conv3", env) == ("basis", "contract")
-    assert f(256, 0, 256, 2, 1723, 862, False, True, "aside", True, False, "enc/conv6", env) == ("basis", "contract")
-    assert f(512, 0, 512, 2, 862, 862, False, True, "aside", True, False, "enc/conv8", env) == ("basis", "fused")
-    # decoder: un-pooling affine blocks contract first, same-level ones stay fused; a precise one contracts first too
+    # encoder: forward fused (every tensor-core contraction accumulates in short chains, so the encoder needs no plain
+    # operands); data gradient: conv2 stays fused (64 wide), conv3 narrows and conv6 pools 256 wide -> contract first,
+    # conv8 (K*F > 512) not
+    assert f(64, 0, 64, 2, 6890, 3445, False, True, "aside", False, "enc/conv2", env) == ("fused", "fused")
+    assert f(64, 0, 128, 2, 3445, 3445, False, True, "aside", False, "enc/conv3", env) == ("fused", "contract")
+    assert f(256, 0, 256, 2, 1723, 862, False, True, "aside", False, "enc/conv6", env) == ("fused", "contract")
+    assert f(512, 0, 512, 2, 862, 862, False, True, "aside", False, "enc/conv8", env) == ("fused", "fused")
+    # decoder: un-pooling affine blocks contract first, same-level ones stay fused
     # (the wide un-pooling block also takes its data gradient basis-first, the narrower ones stay fused)
-    assert f(256, 64, 128, 2, 862, 1723, True, True, "gside", False, False, "dec/aff3", env) == ("contract", "basis")
-    assert f(128, 64, 64, 2, 1723, 3445, True, True, "gside", False, False, "dec/aff5", env) == ("contract", "fused")
-    assert f(512, 64, 256, 2, 862, 862, True, True, "gside", False, False, "dec/aff1", env) == ("fused", "fused")
-    assert f(512, 64, 256, 2, 862, 862, True, True, "gside", True, False, "dec/aff1", env)[0] == "contract"
+    assert f(256, 64, 128, 2, 862, 1723, True, True, "gside", False, "dec/aff3", env) == ("contract", "basis")
+    assert f(128, 64, 64, 2, 1723, 3445, True, True, "gside", False, "dec/aff5", env) == ("contract", "fused")
+    assert f(512, 64, 256, 2, 862, 862, True, True, "gside", False, "dec/aff1", env) == ("fused", "fused")
     # an affine block that WIDENS (32 -> 64: generated 4-layer hierarchies) has two upstream gradients: its data gradient
     # must not take the single-tensor contract-first form, not even on request
-    assert f(32, 64, 64, 2, 3445, 3445, True, True, "aside", False, False, "dec/aff2", env) == ("fused", "fused")
-    assert f(32, 64, 64, 2, 3445, 3445, True, True, "aside", False, False, "dec/aff2", {"CAPE_DX_MODE": "contract"})[1] == "fused"
-    # discriminator (not precise, K = 3, pooled): basis-first forward (the fused kernel's 19-tap gather loses to gather
-    # launch + plain contraction), contract-first data gradient where the layer pools and narrows; the first layer
-    # carries the condition channels and stays fused
-    assert f(64, 0, 128, 3, 1723, 862, False, True, "aside", False, False, "disc/conv3", env) == ("basis", "contract")
-    assert f(64, 0, 64, 3, 3445, 1723, False, True, "aside", False, False, "disc/conv2", env) == ("basis", "fused")
-    assert f(3, 64, 64, 3, 6890, 3445, False, False, "gather", False, False, "disc/conv1", env) == ("fused", "fused")
+    assert f(32, 64, 64, 2, 3445, 3445, True, True, "aside", False, "dec/aff2", env) == ("fused", "fused")
+    assert f(32, 64, 64, 2, 3445, 3445, True, True, "aside", False, "dec/aff2", {"CAPE_DX_MODE": "contract"})[1] == "fused"
+    # discriminator (K = 3, pooled): basis-first forward (the fused kernel's 19-tap gather against gather launch + plain
+    # contraction), contract-first data gradient where the layer pools and narrows; the first layer carries the condition
+    # channels and stays fused
+    assert f(64, 0, 128, 3, 1723, 862, False, True, "aside", False, "disc/conv3", env) == ("basis", "contract")
+    assert f(64, 0, 64, 3, 3445, 1723, False, True, "aside", False, "disc/conv2", env) == ("basis", "fused")
+    assert f(3, 64, 64, 3, 6890, 3445, False, False, "gather", False, "disc/conv1", env) == ("fused", "fused")
     # thin layers and 1x1 convs (identity operators only) never split
-    assert f(3, 0, 64, 2, 6890, 6890, False, False, "gather", True, False, "enc/conv1", env) == ("fused", "fused")
-    assert f(512, 0, 64, 1, 862, 862, False, True, "gside", True, True, "enc/1x1", env) == ("fused", "fused")
+    assert f(3, 0, 64, 2, 6890, 6890, False, False, "gather", False, "enc/conv1", env) == ("fused", "fused")
+    assert f(512, 0, 64, 1, 862, 862, False, True, "gside", True, "enc/1x1", env) == ("fused", "fused")
     # overrides: global and per layer; ineligible requests are ignored
-    assert f(64, 0, 128, 2, 3445, 3445, False, True, "aside", True, False, "enc/conv3", {"CAPE_FWD_MODE": "fused"})[0] == "fused"
-    assert f(512, 0, 512, 2, 862, 862, False, True, "aside", True, False, "enc/conv8",
-             {"CAPE_MODES": "enc/conv8:dx=contract,enc/conv7:fwd=fused"}) == ("basis", "contract")
-    assert f(512, 64, 256, 2, 862, 862, True, True, "gside", False, False, "dec/aff1", {"CAPE_FWD_MODE": "basis"})[0] == "fused"
+    assert f(64, 0, 128, 2, 3445, 3445, False, True, "aside", False, "enc/conv3", {"CAPE_FWD_MODE": "basis"})[0] == "basis"
+    assert f(64, 0, 128, 2, 3445, 3445, False, True, "aside", False, "enc/conv3", {"CAPE_DX_MODE": "fused"})[1] == "fused"
+    assert f(512, 0, 512, 2, 862, 862, False, True, "aside", False, "enc/conv8",
+             {"CAPE_MODES": "enc/conv8:dx=contract,enc/conv7:fwd=basis"}) == ("fused", "contract")
+    assert f(512, 64, 256, 2, 862, 862, True, True, "gside", False, "dec/aff1", {"CAPE_FWD_MODE": "basis"})[0] == "fused"
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_CFG), reason="reference tree not present (GPU box)")
-def test_flag_inventory_is_the_references(monkeypatch):
-    """Every flag the reference's own parse_config declares (config_parser.py:11-63) -- name, type, default, choices --
-    against the table this package parses with.  The reference needs `configargparse` (not installed): a recording
-    stand-in captures its add_argument calls while its unmodified parse_config runs."""
-    import argparse
-    import importlib.util
-    import sys
-    import types
+def test_flag_inventory_is_the_references():
+    """Every flag the reference's own parse_config declares (config_parser.py:11-63) -- name, type, default, choices,
+    recorded by tests/golden/make_host_golden.py while its unmodified parse_config ran -- against the table this
+    package parses with, and the defaults our parser hands out when neither a file nor a flag sets them."""
     from cape_b200 import config_parser as ours
-    recorded = []
-
-    class ArgParser(object):
-        def __init__(self, *a, **k):
-            pass
-
-        def add_argument(self, flag, **kw):
-            recorded.append((flag.lstrip("-"), kw))
-
-        def parse_known_args(self, *a, **k):
-            return argparse.Namespace(**{n: kw.get("default") for n, kw in recorded}), []
-
-    stub = types.ModuleType("configargparse")
-    stub.ArgParser, stub.ArgumentDefaultsHelpFormatter, stub.DefaultConfigFileParser = ArgParser, object, object
-    monkeypatch.setitem(sys.modules, "configargparse", stub)
-    spec = importlib.util.spec_from_file_location("ref_config_parser", os.path.join(os.path.dirname(REF_CFG), "config_parser.py"))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    args, args_dict = mod.parse_config()
-    assert recorded[0][0] == "config" and recorded[0][1]["is_config_file"] and recorded[0][1]["default"] == ours.DEFAULT_CONFIG
-    ref = [(n, kw.get("type", str), kw.get("default"), kw.get("choices")) for n, kw in recorded[1:]]
-    mine = [(n, t, d, ours._CHOICES.get(n)) for n, t, d, _ in ours._SPEC]
+    z = np.load(H.OUT)
+    name, is_cfg, default = z["flags/config"].tolist()
+    assert name == "config" and is_cfg == "True" and default == repr(ours.DEFAULT_CONFIG)
+    ref = list(zip(z["flags/names"].tolist(), z["flags/types"].tolist(), z["flags/defaults"].tolist(),
+                   z["flags/choices"].tolist()))
+    mine = [(n, t.__name__, repr(d), repr(ours._CHOICES.get(n))) for n, t, d, _ in ours._SPEC]
     assert [r[0] for r in ref] == [m[0] for m in mine]                       # same flags, same order
     for r, m in zip(ref, mine):
         assert r == m, (r, m)
-    # and the defaults our parser hands out when neither a file nor a flag sets them
     a, _ = ours.parse_config(["--config", os.devnull])
-    for n, kw in recorded[1:]:
-        assert getattr(a, n) == kw.get("default"), n
+    for n, _, d, _ in ref:
+        assert repr(getattr(a, n)) == d, n

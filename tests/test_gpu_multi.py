@@ -1,7 +1,7 @@
 """Data parallelism on real GPUs (skipped with fewer than two): every rank ends up with the gradients of the GLOBAL
 batch and replicas stay bit-identical -- with the default all-reduce between the two step graphs (eager and
 graph-replayed), and with the bucketed all-reduce inside the step (CapeNetwork.set_data_parallel; opt-in:
-CAPE_TEST_DP_OVERLAP=eager runs it eagerly -- verified on two B200s --, =1 also graph-replayed: that step completes
+CAPE_TEST_DP_OVERLAP=eager runs it eagerly, =1 also graph-replayed: that step completes
 and returns its results, but tearing the process group down afterwards hangs, so it stays off by default)."""
 import os
 import socket

@@ -107,6 +107,12 @@ SIGNATURES = {
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cape_gn_relu_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cape_smpl_create": (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.POINTER(C.c_void_p)]),
+    "cape_smpl_destroy": (None, [C.c_void_p]),
+    "cape_smpl_workspace_bytes": (C.c_int64, [C.c_void_p, C.c_int]),
+    "cape_smpl_pose": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                 C.c_void_p]),
 }
 
 _lib = None

@@ -348,6 +348,45 @@ def resample(tp, op, x, y, N, rows_out, rows_in, F, x_stride=None, y_stride=None
                                cond.shape[1] if cond is not None else 0, _stream()))
 
 
+class SmplPoser:
+    """Owns a cape_smpl handle: an SMPL body model resident on one device that poses batches of meshes [N, V, 3] with
+    poses [N, 72] (cape_smpl_pose; the scratch is a torch buffer kept between calls)."""
+
+    def __init__(self, jreg_ptr, jreg_col, jreg_val, posedirs, weights, parents, device=0):
+        self.lib = _lib.load()
+        if not torch.cuda.is_available():
+            raise _lib.CapeError("cape_b200 needs a CUDA device: there is no CPU execution path")
+        self.device = torch.device("cuda", device if isinstance(device, int) else device.index or 0)
+        self.V = int(weights.shape[0])
+        host = [np.ascontiguousarray(jreg_ptr, np.int32), np.ascontiguousarray(jreg_col, np.int32),
+                np.ascontiguousarray(jreg_val, np.float32), np.ascontiguousarray(posedirs, np.float32),
+                np.ascontiguousarray(weights, np.float32), np.ascontiguousarray(parents, np.int32)]
+        h = C.c_void_p()
+        check(self.lib.cape_smpl_create(self.device.index, self.V, *[a.ctypes.data_as(C.c_void_p) for a in host],
+                                        C.byref(h)))
+        self.h = h
+        self.ws = torch.empty(0, dtype=torch.uint8, device=self.device)
+
+    def __del__(self):
+        try:
+            if getattr(self, "h", None):
+                self.lib.cape_smpl_destroy(self.h)
+                self.h = None
+        except Exception:
+            pass
+
+    def pose(self, verts, pose, out):
+        """out[n] = verts[n] posed with pose[n]; fp32 CUDA tensors [N, V, 3], [N, 72], [N, V, 3]."""
+        N = verts.shape[0]
+        assert verts.shape == (N, self.V, 3) and pose.shape == (N, 72) and out.shape == verts.shape
+        assert verts.is_contiguous() and pose.is_contiguous() and out.is_contiguous()
+        nbytes = check(self.lib.cape_smpl_workspace_bytes(self.h, N))
+        if self.ws.numel() < nbytes:
+            self.ws = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        check(self.lib.cape_smpl_pose(self.h, N, _ptr(_f32(verts)), _ptr(_f32(pose)), _ptr(_f32(out)), _ptr(self.ws),
+                                      self.ws.numel(), _stream()))
+
+
 def gn_relu_fwd(tp, x, gamma, beta, y, stats, G, eps=1e-5):
     N, rows, Cc = x.shape
     check(tp.lib.cape_gn_relu_fwd(tp.h, _ptr(x), N, rows, Cc, G, eps, _ptr(gamma), _ptr(beta), _ptr(y), _ptr(stats),

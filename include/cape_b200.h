@@ -320,6 +320,25 @@ int cape_gn_relu_bwd(cape_topology* t, const float* x, const float* y, const flo
                      const float* gamma, const float* stats, float* dx, int accumulate_dx, float* dgamma, float* dbeta,
                      void* stream);
 
+/* ---- SMPL posing (demo_full's pose_result, demos.py:249-331: smplx.lbs with zero betas) -----------------------------
+ * A device-resident SMPL body model with the template replaced per call, as the reference does: every mesh verts[n] is
+ * posed with pose[n] (24 axis-angle vectors, global orientation first):
+ *   J = J_regressor . verts[n]  (joints of the given mesh),  R_j = Rodrigues(pose[n, j]),
+ *   v_posed = verts[n] + (R_1..23 - I) . posedirs,  G_j = G_parent(j) . [R_j | J_j - J_parent(j)],
+ *   out[n, v] = sum_j weights[v, j] (G_j - G_j . [J_j, 0]) . [v_posed, 1].
+ * cape_smpl_create copies the model to `device`: J_regressor as CSR (jreg_ptr [25], jreg_col / jreg_val [jreg_ptr[24]],
+ * columns < V), posedirs [207, V * 3] (element (p, 3 v + c) = the pickle's posedirs[v, c, p]), weights [V, 24] (kept as
+ * each vertex's non-zero entries) and parents [24] (parents[0] = -1, 0 <= parents[j] < j).  cape_smpl_pose takes fp32
+ * device tensors verts / out [N, V, 3] and pose [N, 72], and scratch of cape_smpl_workspace_bytes(s, N) bytes
+ * (16-byte aligned).  Three launches on `stream`; the pose-blend product runs on cape_gemm. */
+typedef struct cape_smpl cape_smpl;
+int cape_smpl_create(int device, int V, const int32_t* jreg_ptr, const int32_t* jreg_col, const float* jreg_val,
+                     const float* posedirs, const float* weights, const int32_t* parents, cape_smpl** out);
+void cape_smpl_destroy(cape_smpl* s);
+int64_t cape_smpl_workspace_bytes(const cape_smpl* s, int N);
+int cape_smpl_pose(cape_smpl* s, int N, const float* verts, const float* pose, float* out, void* workspace,
+                   int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

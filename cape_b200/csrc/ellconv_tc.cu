@@ -6,11 +6,21 @@
 // with fp32 accuracy by 3xTF32 error compensation:  a = a_hi + a_lo (a_hi = top 19 bits, a_lo = the exact remainder),
 // acc += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo with fp32 accumulation; the dropped a_lo*b_lo term is ~2^-22 relative.
 //
-// A CTA of two warpgroups owns one 128-row x BN-column output tile (grid.y walks the column tiles).  All 256 threads
-// gather the Chebyshev-basis chunk A[128 rows x 32 k] from neighbour rows (float4 loads, same ELL tables as the SIMT
-// path) and load the weight chunk B[BN x 32 k] (K-major copy of W), split both into hi/lo and store them in the
-// swizzled K-major layout; each warpgroup then issues wgmma m64nBNk8 for its 64 rows.  The shared-memory tiles are
-// double-buffered: the loads of chunk j+1 are in flight while the MMAs of chunk j run.
+// A CTA owns one 128-row x BN-column output tile and runs four warpgroups around a ring of shared-memory stages:
+//  - warpgroups 0 and 1, the producers, gather the Chebyshev-basis chunk A[128 rows x 32 k] from neighbour rows
+//    (float4 loads, same ELL tables and row mapping as the SIMT path) or load it from a plain operand, load the weight
+//    chunk B[BN x 32 k] (K-major copy of W), split both into hi/lo and store them in the swizzled K-major layout of the
+//    next free stage, then arrive on the stage's `full` mbarrier;
+//  - warpgroups 2 and 3, the consumers, each own 64 output rows: wait on `full`, issue wgmma m64nBNk8 for the chunk,
+//    wait for it, add the chunk's sum into the running accumulator and release the stage on its `empty` mbarrier.
+// The producers run up to STAGES chunks ahead, so the gather of later chunks overlaps the MMAs of earlier ones, and the
+// two consumers never wait for each other.  setmaxnreg moves registers from the producers to the consumers, which hold
+// the accumulators.  Two producer warpgroups, not one, and each producer thread gathers both of its row pairs at
+// once (16 neighbour-row loads in flight) with the weight chunk's loads issued first: the gather is latency-bound
+// on L2, and fewer loads in flight than the 256-thread lockstep kernel this replaces made the gather-heavy layers
+// slower on the H100.
+// The grid is 1-D with the column tiles fastest, so the CTAs of one row tile run together and read its source rows
+// from L2 rather than from HBM once per column tile.
 //
 // Every chunk's products go to a fresh register accumulator that is added to the running sum in fp32 with
 // round-to-nearest, so the tensor core's truncating accumulation chain is one chunk (12 MMAs) long instead of the whole
@@ -26,33 +36,208 @@ namespace {
 
 using namespace tc;
 
-constexpr int WG_THREADS = 256;
+constexpr int CONV_THREADS = 512;             // two producer warpgroups + two consumer warpgroups
+constexpr int PRODUCER_THREADS = 256;
+constexpr int CONSUMER_THREADS = 256;
+// per-thread registers after setmaxnreg: 256 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 512 * 128 (the launch budget
+// of a 512-thread CTA)
+constexpr int PRODUCER_REGS = 112;
+constexpr int CONSUMER_REGS = 144;
+constexpr int GATHER_PAIRS = 2;               // row pairs each producer thread gathers at once
 constexpr int A_TILE = BM * 128;              // 128 rows x 32 fp32
 constexpr int QS_MAX_FLOATS = 8192;           // condition vectors of the tile's samples and columns
+constexpr int BAR_BYTES = 256;                // the ring's mbarriers
+constexpr int SMEM_MAX = 227 * 1024;          // dynamic shared memory per CTA on sm_90
 
 template <int BN, bool DUAL>
 struct ConvCfg {
   static constexpr int B_TILE = BN * 128;
   static constexpr int STAGE = 2 * A_TILE + (DUAL ? 4 : 2) * B_TILE;
-  static constexpr int RING = 2 * STAGE;
+  // as many stages (up to 4) as fit beside the largest condition-vector buffer
+  static constexpr int FIT = (SMEM_MAX - 1024 - BAR_BYTES - QS_MAX_FLOATS * 4) / STAGE;
+  static constexpr int STAGES = FIT < 4 ? FIT : 4;
+  static constexpr int RING = STAGES * STAGE;
+  static_assert(STAGES >= 3, "the ring needs at least three stages");
+  static_assert(2 * STAGES * 8 <= BAR_BYTES, "mbarrier area too small");
 };
 
+// Gathers rows (ra[i], rb[i]) for NP pairs: the producers' copy of ell_gather4_pair (NP = 1), which this one matches
+// tap for tap; written for NP pairs at once so that more loads can be put in flight when registers allow.  Each
+// pair stops when both of its rows are exhausted, and an exhausted row of a live pair adds 0 * (row 0), exactly as
+// ell_gather4_pair does for one pair.
+template <int NP>
+__device__ __forceinline__ void ell_gather4_pairs(const OpView& op, const int (&ra)[NP], const int (&rb)[NP],
+                                                  const float* (&base_a)[NP], const float* (&base_b)[NP],
+                                                  size_t stride, float4 (&va)[NP], float4 (&vb)[NP]) {
+  const int nb = op.width >> 2;
+  int4 ia[NP], ib[NP];
+#pragma unroll
+  for (int q = 0; q < NP; ++q) {
+    ia[q] = __ldg(reinterpret_cast<const int4*>(op.idx + (size_t)ra[q] * op.width));
+    ib[q] = __ldg(reinterpret_cast<const int4*>(op.idx + (size_t)rb[q] * op.width));
+  }
+  for (int b = 0; b < nb; ++b) {
+    bool any = false;
+#pragma unroll
+    for (int q = 0; q < NP; ++q) any |= ia[q].x >= 0 || ib[q].x >= 0;
+    if (!any) break;
+#pragma unroll
+    for (int q = 0; q < NP; ++q) {
+      const bool da = ia[q].x >= 0, db = ib[q].x >= 0;
+      if (!da && !db) continue;
+      float4 wa = make_float4(0.f, 0.f, 0.f, 0.f), wb = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (da) wa = __ldg(reinterpret_cast<const float4*>(op.w + (size_t)ra[q] * op.width) + b);
+      if (db) wb = __ldg(reinterpret_cast<const float4*>(op.w + (size_t)rb[q] * op.width) + b);
+      int4 na = make_int4(-1, -1, -1, -1), nbx = make_int4(-1, -1, -1, -1);
+      if (b + 1 < nb) {
+        na = __ldg(reinterpret_cast<const int4*>(op.idx + (size_t)ra[q] * op.width) + b + 1);
+        nbx = __ldg(reinterpret_cast<const int4*>(op.idx + (size_t)rb[q] * op.width) + b + 1);
+      }
+      const float* pa = base_a[q];
+      const float* pb = base_b[q];
+      const float4 a0 = ldg4(pa + (size_t)max(ia[q].x, 0) * stride), a1 = ldg4(pa + (size_t)max(ia[q].y, 0) * stride);
+      const float4 a2 = ldg4(pa + (size_t)max(ia[q].z, 0) * stride), a3 = ldg4(pa + (size_t)max(ia[q].w, 0) * stride);
+      const float4 b0 = ldg4(pb + (size_t)max(ib[q].x, 0) * stride), b1 = ldg4(pb + (size_t)max(ib[q].y, 0) * stride);
+      const float4 b2 = ldg4(pb + (size_t)max(ib[q].z, 0) * stride), b3 = ldg4(pb + (size_t)max(ib[q].w, 0) * stride);
+      fma4(va[q], wa.x, a0); fma4(va[q], wa.y, a1); fma4(va[q], wa.z, a2); fma4(va[q], wa.w, a3);
+      fma4(vb[q], wb.x, b0); fma4(vb[q], wb.y, b1); fma4(vb[q], wb.z, b2); fma4(vb[q], wb.w, b3);
+      ia[q] = na; ib[q] = nbx;
+    }
+  }
+}
+
 template <int BN, bool DUAL>
-__global__ void __launch_bounds__(WG_THREADS, BN <= 32 && !DUAL ? 2 : 1) conv_wg_kernel(const __grid_constant__ ConvParams p, int nqs) {
+__global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_constant__ ConvParams p, int nqs,
+                                                                  int ncol_tiles) {
   using Cfg = ConvCfg<BN, DUAL>;
-  constexpr int NA = BN / 2;                  // accumulator registers per thread
+  constexpr int S = Cfg::STAGES;
+  constexpr int NA = BN / 2;                  // accumulator registers per consumer thread
   extern __shared__ uint8_t smem_raw[];
   char* smem = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  float* qs = reinterpret_cast<float*>(smem + Cfg::RING);
+  uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::RING);
+  uint64_t* empty = full + S;
+  float* qs = reinterpret_cast<float*>(smem + Cfg::RING + BAR_BYTES);
 
-  const int tid = threadIdx.x, wgi = tid >> 7, wt = tid & 127;
-  const long long row0 = (long long)blockIdx.x * BM;
-  const int col0 = blockIdx.y * BN;
-  const int n_first = (int)(row0 / p.rows_out);
+  const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
+  const int ct = (int)(blockIdx.x % (unsigned)ncol_tiles);
+  const long long row0 = (long long)(blockIdx.x / (unsigned)ncol_tiles) * BM;
+  const int col0 = ct * BN;
+
+  // the reduction: 32-deep chunks over all terms (a term of F = 0 still takes one all-zero chunk)
+  int nchunks = 0;
+  for (int t = 0; t < p.nterms; ++t) nchunks += max(1, (p.terms[t].F + BK - 1) / BK);
+
+  if (tid == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(&full[s], PRODUCER_THREADS);  // every producer thread
+      mbar_init(&empty[s], 8);                // one lane per consumer warp
+    }
+  }
+  __syncthreads();
+
+  if (tid < PRODUCER_THREADS) {
+    // =========================== producers ===========================
+    setmaxnreg_dec<PRODUCER_REGS>();
+    // 8 threads per 128-byte tile row (one float4 of k each), 32 row slots; rows rs + 32 i, gathered in the pairs
+    // (rs, rs + 32) and (rs + 64, rs + 96): the row mapping of the SIMT kernels, so each row's taps add in their order
+    const int l8 = tid & 7, rs = tid >> 3;
+    constexpr int ROWS[4] = {0, 32, 64, 96};
+    int rn[4], rr[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const long long R = row0 + rs + ROWS[i];
+      if (R < p.total_rows) { rn[i] = (int)(R / p.rows_out); rr[i] = (int)(R % p.rows_out); }
+      else { rn[i] = -1; rr[i] = 0; }
+    }
+    const bool do_stash = ct == 0;            // one column tile writes the basis copies
+    int t = 0, f0 = 0;
+    for (int j = 0; j < nchunks; ++j) {
+      const int stage = j % S;
+      mbar_wait(&empty[stage], ((j / S) & 1) ^ 1);
+      char* a_hi = smem + (size_t)stage * Cfg::STAGE;
+      char* a_lo = a_hi + A_TILE;
+      char* b_hi = a_lo + A_TILE;
+      char* b_lo = b_hi + Cfg::B_TILE;
+      const TermDev& tm = p.terms[t];
+      const int f = f0 + l8 * 4;
+      // the weight chunk's loads first: they are independent of the gather and fly while it runs
+      const bool has2 = DUAL && tm.w2T != nullptr;
+      float4 rb[BN / 32], rb2[DUAL ? BN / 32 : 1];
+#pragma unroll
+      for (int i = 0; i < BN / 32; ++i) {
+        const int c = col0 + rs + 32 * i;
+        rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (c < p.ncols && f < tm.F) rb[i] = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
+        if (DUAL) {
+          rb2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (has2 && c < p.ncols && f < tm.F) rb2[i] = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
+        }
+      }
+#pragma unroll
+      for (int h = 0; h < 2 / GATHER_PAIRS; ++h) {  // GATHER_PAIRS pairs (ROWS[2q], ROWS[2q + 1]) at a time
+        constexpr int NP = GATHER_PAIRS;
+        float4 va[NP], vb[NP];
+#pragma unroll
+        for (int q = 0; q < NP; ++q) { va[q] = make_float4(0.f, 0.f, 0.f, 0.f); vb[q] = va[q]; }
+        if (f < tm.F) {
+          // invalid (beyond-the-end) rows gather sample 0 / row 0 and are zeroed afterwards
+          const float* base_a[NP];
+          const float* base_b[NP];
+          int ra[NP], rb_[NP];
+#pragma unroll
+          for (int q = 0; q < NP; ++q) {
+            const int ia = 2 * (h * NP + q);
+            base_a[q] = tm.src + (size_t)max(rn[ia], 0) * tm.src_rows * tm.src_stride + f;
+            base_b[q] = tm.src + (size_t)max(rn[ia + 1], 0) * tm.src_rows * tm.src_stride + f;
+            ra[q] = rr[ia]; rb_[q] = rr[ia + 1];
+          }
+          if (tm.op.idx == nullptr) {
+#pragma unroll
+            for (int q = 0; q < NP; ++q) {
+              va[q] = ldg4(base_a[q] + (size_t)ra[q] * tm.src_stride);
+              vb[q] = ldg4(base_b[q] + (size_t)rb_[q] * tm.src_stride);
+            }
+          } else {
+            ell_gather4_pairs<NP>(tm.op, ra, rb_, base_a, base_b, (size_t)tm.src_stride, va, vb);
+          }
+        }
+#pragma unroll
+        for (int q = 0; q < NP; ++q) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int i = 2 * (h * NP + q) + e;
+            float4 v = e == 0 ? va[q] : vb[q];
+            if (rn[i] < 0) v = make_float4(0.f, 0.f, 0.f, 0.f);
+            const int row = rs + ROWS[i];
+            if (f < tm.F && tm.stash != nullptr && do_stash && rn[i] >= 0)   // basis rows for the weight gradient
+              *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row) * tm.stash_stride + f) = v;
+            split_store4(v, a_hi, a_lo, (uint32_t)(row * 128 + ((l8 ^ (row & 7)) << 4)));
+          }
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < BN / 32; ++i) {
+        const int cl = rs + 32 * i;
+        const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
+        split_store4(rb[i], b_hi, b_lo, off);
+        if (DUAL) split_store4(rb2[i], b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, off);
+      }
+      fence_proxy_async();                    // generic-proxy smem writes -> visible to the tensor core's (async) proxy
+      mbar_arrive(&full[stage]);
+      f0 += BK;
+      if (f0 >= tm.F) { f0 = 0; ++t; }
+    }
+    return;
+  }
+
+  // =========================== consumers ===========================
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const int cw = wg - 2, ctid = tid - PRODUCER_THREADS;
 
   // condition broadcast vectors of this tile: qs[s][slot][c] = cond[n_first + s, :] . Wc_slot[:, col0 + c]
+  const int n_first = (int)(row0 / p.rows_out);
   if (p.nslots > 0) {
-    for (int o = tid; o < nqs; o += WG_THREADS) {
+    for (int o = ctid; o < nqs; o += CONSUMER_THREADS) {
       const int c = o % BN, slot = (o / BN) % p.nslots, s = o / (BN * p.nslots);
       float q = 0.f;
       const int n = n_first + s;
@@ -66,88 +251,14 @@ __global__ void __launch_bounds__(WG_THREADS, BN <= 32 && !DUAL ? 2 : 1) conv_wg
     }
   }
 
-  // producer mapping: 8 threads per 128-byte tile row (one float4 of k each), 32 row slots
-  const int l8 = tid & 7, rs = tid >> 3;
-  int rn[4], rr[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const long long R = row0 + rs + 32 * i;
-    if (R < p.total_rows) { rn[i] = (int)(R / p.rows_out); rr[i] = (int)(R % p.rows_out); }
-    else { rn[i] = -1; rr[i] = 0; }
-  }
-  const bool do_stash = blockIdx.y == 0;      // one column tile writes the basis copies
-
-  float4 ra[4], rb[BN / 32], rb2[DUAL ? BN / 32 : 1];
-
-  auto load_chunk = [&](int t, int f0) {
-    const TermDev& tm = p.terms[t];
-    const int f = f0 + l8 * 4;
-#pragma unroll
-    for (int i = 0; i < 4; i += 2) {
-      float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (f < tm.F) {
-        // invalid (beyond-the-end) rows gather sample 0 / row 0 and are zeroed afterwards
-        const float* base_a = tm.src + (size_t)max(rn[i], 0) * tm.src_rows * tm.src_stride + f;
-        const float* base_b = tm.src + (size_t)max(rn[i + 1], 0) * tm.src_rows * tm.src_stride + f;
-        if (tm.op.idx == nullptr) {
-          a = ldg4(base_a + (size_t)rr[i] * tm.src_stride);
-          b = ldg4(base_b + (size_t)rr[i + 1] * tm.src_stride);
-        } else {
-          ell_gather4_pair(tm.op, rr[i], rr[i + 1], base_a, base_b, (size_t)tm.src_stride, a, b);
-        }
-        if (rn[i] < 0) a = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (rn[i + 1] < 0) b = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (tm.stash != nullptr && do_stash) {    // keep the basis rows for the weight gradient (cape_term.stash)
-          if (rn[i] >= 0) *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + rs + 32 * i) * tm.stash_stride + f) = a;
-          if (rn[i + 1] >= 0)
-            *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + rs + 32 * i + 32) * tm.stash_stride + f) = b;
-        }
-      }
-      ra[i] = a; ra[i + 1] = b;
-    }
-    const bool has2 = DUAL && tm.w2T != nullptr;
-#pragma unroll
-    for (int i = 0; i < BN / 32; ++i) {
-      const int c = col0 + rs + 32 * i;
-      rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (c < p.ncols && f < tm.F) rb[i] = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
-      if (DUAL) {
-        rb2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (has2 && c < p.ncols && f < tm.F) rb2[i] = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
-      }
-    }
-  };
-  auto store_chunk = [&](int stage) {
-    char* a_hi = smem + (size_t)stage * Cfg::STAGE;
-    char* a_lo = a_hi + A_TILE;
-    char* b_hi = a_lo + A_TILE;
-    char* b_lo = b_hi + Cfg::B_TILE;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int row = rs + 32 * i;
-      split_store4(ra[i], a_hi, a_lo, (uint32_t)(row * 128 + ((l8 ^ (row & 7)) << 4)));
-    }
-#pragma unroll
-    for (int i = 0; i < BN / 32; ++i) {
-      const int cl = rs + 32 * i;
-      const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
-      split_store4(rb[i], b_hi, b_lo, off);
-      if (DUAL) split_store4(rb2[i], b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, off);
-    }
-  };
-
   float acc0[NA], acc1[DUAL ? NA : 1], part0[NA], part1[DUAL ? NA : 1];
 #pragma unroll
   for (int i = 0; i < NA; ++i) { acc0[i] = 0.f; if (DUAL) acc1[i] = 0.f; }
 
-  // the reduction: 32-deep chunks over all terms
-  int t = 0, f0 = 0;
-  load_chunk(0, 0);
-  store_chunk(0);
-  fence_proxy_async();
-  __syncthreads();
-  for (int j = 0, stage = 0;; ++j, stage ^= 1) {
-    const uint32_t a_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + (uint32_t)(wgi * 64 * 128);
+  for (int j = 0; j < nchunks; ++j) {
+    const int stage = j % S;
+    mbar_wait(&full[stage], (j / S) & 1);
+    const uint32_t a_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + (uint32_t)(cw * 64 * 128);
     const uint32_t a_lo = a_hi + A_TILE;
     const uint32_t b_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + 2 * A_TILE;
     const uint32_t b_lo = b_hi + Cfg::B_TILE;
@@ -159,15 +270,8 @@ __global__ void __launch_bounds__(WG_THREADS, BN <= 32 && !DUAL ? 2 : 1) conv_wg
       mma3_chunk<BN>(part1, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
     }
     wgmma_commit();
-    // next chunk: its loads fly while the MMAs run; the other stage was released at the end of the previous pass
-    f0 += BK;
-    if (f0 >= p.terms[t].F) { f0 = 0; ++t; }
-    const bool more = t < p.nterms;
-    if (more) {
-      load_chunk(t, f0);
-      store_chunk(stage ^ 1);
-    }
     wgmma_wait_all();
+    if ((tid & 31) == 0) mbar_arrive(&empty[stage]);   // this warp's MMAs have read the stage
     fence_acc(part0);
 #pragma unroll
     for (int i = 0; i < NA; ++i) acc0[i] += part0[i];
@@ -176,18 +280,15 @@ __global__ void __launch_bounds__(WG_THREADS, BN <= 32 && !DUAL ? 2 : 1) conv_wg
 #pragma unroll
       for (int i = 0; i < NA; ++i) acc1[i] += part1[i];
     }
-    if (!more) break;
-    fence_proxy_async();            // generic-proxy smem writes -> visible to the tensor core's (async) proxy
-    __syncthreads();                // both warpgroups done with this stage, the next one complete
   }
-  __syncthreads();                  // qs complete (written before the main loop, read below)
+  named_bar_sync(1, CONSUMER_THREADS);        // qs complete (written before the main loop, read below)
 
   // =========================== epilogue: straight from the accumulator registers ===========================
   const bool linear = p.epilogue == CAPE_EPI_LINEAR;
   const bool use_aux = p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {                       // the thread's two rows
-    const int lrow = wgi * 64 + frag_row(wt, 2 * h);
+    const int lrow = cw * 64 + frag_row(wt, 2 * h);
     const long long R = row0 + lrow;
     if (R >= p.total_rows) continue;
     const int n = (int)(R / p.rows_out), r = (int)(R % p.rows_out);
@@ -258,15 +359,21 @@ int launch_conv(const ConvParams& p, cudaStream_t st) {
     const int S = (int)(rlast_max / p.rows_out) + 2;
     nqs = S * p.nslots * BN;
   }
-  const int smem = 1024 + Cfg::RING + nqs * 4;
+  const int smem = 1024 + Cfg::RING + BAR_BYTES + nqs * 4;
   static bool configured = false;
   if (!configured) {
     CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         1024 + Cfg::RING + QS_MAX_FLOATS * 4));
+                                         1024 + Cfg::RING + BAR_BYTES + QS_MAX_FLOATS * 4));
     configured = true;
   }
-  dim3 grid((unsigned)((p.total_rows + BM - 1) / BM), (unsigned)((p.ncols + BN - 1) / BN));
-  conv_wg_kernel<BN, DUAL><<<grid, WG_THREADS, smem, st>>>(p, nqs);
+  // 1-D grid, column tiles fastest (no 65,535 limit on the row tiles)
+  const int ncol_tiles = (p.ncols + BN - 1) / BN;
+  const long long nblocks = (p.total_rows + BM - 1) / BM * ncol_tiles;
+  if (nblocks >= (1LL << 31)) {
+    set_error("conv_wg_kernel: too many tiles");
+    return -1;
+  }
+  conv_wg_kernel<BN, DUAL><<<(unsigned)nblocks, CONV_THREADS, smem, st>>>(p, nqs, ncol_tiles);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;

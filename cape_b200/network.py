@@ -6,6 +6,8 @@ every layer is one (or a few) calls into libcape_b200.so.  Names in comments ref
 encoder :514-561, decoder_cond_vert :564-617, res_block_affine :776-793, res_block_decoder :744-774,
 discriminator :648-678, loss :354-416, training :419-474.
 """
+import contextlib
+import gc
 import math
 import os
 
@@ -1181,15 +1183,31 @@ class CapeNetwork:
         slot[0], slot[1] = lr_g, lr_d
         self.lr.copy_(slot, non_blocking=True)
 
+    @staticmethod
+    @contextlib.contextmanager
+    def _no_collector():
+        """Stream capture with Python's cyclic garbage collector held off.  A dead network it finds mid-capture would
+        destroy its topology handles, and the cudaFree of that invalidates the capture; so dead cycles are collected
+        first, while that is still safe."""
+        gc.collect()
+        was_enabled = gc.isenabled()
+        gc.disable()
+        try:
+            yield
+        finally:
+            if was_enabled:
+                gc.enable()
+
     def capture_graphs(self):
         """Capture forward/backward and the update into two CUDA graphs (the gradient all-reduce runs between
         them).  One eager step must have run before (lazy initialisations, workspace growth)."""
         self.graph_fb, self.graph_up = torch.cuda.CUDAGraph(), torch.cuda.CUDAGraph()
         torch.cuda.synchronize()
-        with torch.cuda.graph(self.graph_fb):
-            self.enqueue_fwd_bwd()
-        with torch.cuda.graph(self.graph_up):
-            self.enqueue_update()
+        with self._no_collector():
+            with torch.cuda.graph(self.graph_fb):
+                self.enqueue_fwd_bwd()
+            with torch.cuda.graph(self.graph_up):
+                self.enqueue_update()
         torch.cuda.synchronize()
 
     def capture_forward_graph(self):
@@ -1197,8 +1215,9 @@ class CapeNetwork:
         CUDA graph: `graph_fwd.replay()` then maps the staged inputs to `x_hat`."""
         self.graph_fwd = torch.cuda.CUDAGraph()
         torch.cuda.synchronize()
-        with torch.cuda.graph(self.graph_fwd):
-            self.forward_generator()
+        with self._no_collector():
+            with torch.cuda.graph(self.graph_fwd):
+                self.forward_generator()
         torch.cuda.synchronize()
 
     def train_step(self, step=None, update=True, allreduce=None, use_graph=False):

@@ -145,7 +145,8 @@ __device__ __forceinline__ void mac_tile(const float* As, const float* Ws, int t
   }
 }
 
-template <int BN, bool DUAL>
+// PASS: the call has pass-through terms (see conv_wg_kernel)
+template <int BN, bool DUAL, bool PASS>
 __global__ void __launch_bounds__(NT, DUAL ? 1 : 2) ellconv_kernel(const __grid_constant__ ConvParams p) {
   constexpr int TX = BN / 4, TY = NT / TX, RPT = BM / TY;
   constexpr int WPT = BK * BN / NT;
@@ -261,6 +262,15 @@ __global__ void __launch_bounds__(NT, DUAL ? 1 : 2) ellconv_kernel(const __grid_
       }
     }
     const int c0 = col0 + tx * 4;
+    if constexpr (PASS) {
+      for (int q = p.nterms; q < p.nterms + p.npass; ++q) {   // pass-through terms (F == ncols)
+        const TermDev& tm = p.terms[q];
+        const float* base = tm.src + (size_t)n * tm.src_rows * tm.src_stride;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (c0 + j < p.ncols) v0[j] += pass_row(tm.op, r, base + c0 + j, (size_t)tm.src_stride);
+      }
+    }
     const size_t obase = ((size_t)(row0 + row)) * p.ncols + c0;
     float o1[4], o2[4];
     bool write2 = false;
@@ -671,11 +681,33 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
   bool dual = false, any_stash = false;
   bool wvec = (a->ncols % 4 == 0);
   p.nslots = 0;
+  // contracted terms first, in call order; pass-through terms (no weights at all) after them
+  int npass = 0;
   for (int i = 0; i < a->nterms; ++i) {
     const cape_term& s = a->terms[i];
+    if (s.w || s.w2 || s.wT || s.w2T) continue;
+    CAPE_REQUIRE(!a->plain_only, "a pass-through term (no w, w2, wT or w2T) cannot be part of a plain_only call");
+    CAPE_REQUIRE(s.src && s.F == a->ncols, "a pass-through term needs src and F == ncols");
+    CAPE_REQUIRE(!s.wc && !s.wc2 && !s.stash, "a pass-through term takes no wc, wc2 or stash");
+    CAPE_REQUIRE(s.src_stride >= s.F, "bad strides");
+    ++npass;
+  }
+  CAPE_REQUIRE(npass < a->nterms, "a call needs at least one contracted term");
+  p.nterms = a->nterms - npass;
+  p.npass = npass;
+  for (int i = 0, ic = 0, ip = p.nterms; i < a->nterms; ++i) {
+    const cape_term& s = a->terms[i];
+    if (!(s.w || s.w2 || s.wT || s.w2T)) {
+      TermDev& d = p.terms[ip++];
+      if (get_op(t, s.op, a->rows_out, s.src_rows, &d.op) != 0) return -1;
+      d.src = s.src; d.F = s.F; d.src_rows = s.src_rows; d.src_stride = s.src_stride;
+      d.vec = (s.F % 4 == 0) && (s.src_stride % 4 == 0) && aligned16(s.src);
+      continue;
+    }
     CAPE_REQUIRE(s.src && (s.w || a->plain_only) && s.F > 0, "term needs src, w and F > 0");
     CAPE_REQUIRE(s.src_stride >= s.F && (s.w_stride >= a->ncols || a->plain_only), "bad strides");
-    TermDev& d = p.terms[i];
+    const int ti = ic++;
+    TermDev& d = p.terms[ti];
     if (get_op(t, s.op, a->rows_out, s.src_rows, &d.op) != 0) return -1;
     d.src = s.src; d.F = s.F; d.src_rows = s.src_rows; d.src_stride = s.src_stride; d.w_stride = s.w_stride; d.w2_stride = s.w2_stride;
     d.w = s.w; d.w2 = s.w2;
@@ -696,11 +728,11 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
     }
     if (s.wc) {
       CAPE_REQUIRE(a->cond && a->C > 0, "condition weights without cond");
-      p.slot_term[p.nslots] = i; p.slot_acc[p.nslots] = 0; p.slot_w[p.nslots] = s.wc; ++p.nslots;
+      p.slot_term[p.nslots] = ti; p.slot_acc[p.nslots] = 0; p.slot_w[p.nslots] = s.wc; ++p.nslots;
     }
     if (s.wc2) {
       CAPE_REQUIRE(a->cond && a->C > 0 && s.w2, "wc2 needs cond and w2");
-      p.slot_term[p.nslots] = i; p.slot_acc[p.nslots] = 1; p.slot_w[p.nslots] = s.wc2; ++p.nslots;
+      p.slot_term[p.nslots] = ti; p.slot_acc[p.nslots] = 1; p.slot_w[p.nslots] = s.wc2; ++p.nslots;
     }
   }
   p.cond = a->cond; p.C = a->C;
@@ -735,7 +767,7 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
     if (rc != 0) return rc < 0 ? rc : 0;
   }
   if (any_stash) {                                        // fp32-pipe path: the basis copies come from the resample kernel
-    for (int i = 0; i < a->nterms; ++i) {
+    for (int i = 0; i < p.nterms; ++i) {
       const TermDev& d = p.terms[i];
       if (!d.stash) continue;
       const long long blocks = (p.total_rows * 32 + 255) / 256;
@@ -747,12 +779,20 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
     }
   }
   dim3 grid((unsigned)((p.total_rows + BM - 1) / BM), (unsigned)((a->ncols + BNsel - 1) / BNsel));
-  if (dual) {
-    if (BNsel == 32) ellconv_kernel<32, true><<<grid, NT, 0, st>>>(p);
-    else ellconv_kernel<64, true><<<grid, NT, 0, st>>>(p);
+  if (p.npass > 0) {
+    if (dual) {
+      if (BNsel == 32) ellconv_kernel<32, true, true><<<grid, NT, 0, st>>>(p);
+      else ellconv_kernel<64, true, true><<<grid, NT, 0, st>>>(p);
+    } else {
+      if (BNsel == 32) ellconv_kernel<32, false, true><<<grid, NT, 0, st>>>(p);
+      else ellconv_kernel<64, false, true><<<grid, NT, 0, st>>>(p);
+    }
+  } else if (dual) {
+    if (BNsel == 32) ellconv_kernel<32, true, false><<<grid, NT, 0, st>>>(p);
+    else ellconv_kernel<64, true, false><<<grid, NT, 0, st>>>(p);
   } else {
-    if (BNsel == 32) ellconv_kernel<32, false><<<grid, NT, 0, st>>>(p);
-    else ellconv_kernel<64, false><<<grid, NT, 0, st>>>(p);
+    if (BNsel == 32) ellconv_kernel<32, false, false><<<grid, NT, 0, st>>>(p);
+    else ellconv_kernel<64, false, false><<<grid, NT, 0, st>>>(p);
   }
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);

@@ -41,12 +41,47 @@ struct ConvParams {
   float alpha;
   const float* bias;
   int bias_per_row;
+  // terms[0, nterms) are contracted; terms[nterms, nterms + npass) are pass-through terms (cape_term with no weights:
+  // acc0 += op . src[:, :, :ncols] in the epilogue).  A launcher that does not add them must decline a call with npass > 0.
+  // (Here it fills the padding before `aux`: the layout of the other fields is unchanged.)
+  int npass;
   const float* aux;
   float* out;
   float* out2;
   int wvec, ovec;
 };
 
+// One row of a pass-through term: sum_j op[r, j] * base[idx[r, j] * stride] (op.idx == nullptr: base[r * stride]), taps in
+// table order.  `base` points at the sample's source rows, offset by the column.
+__device__ __forceinline__ float pass_row(const OpView& op, int r, const float* base, size_t stride) {
+  if (op.idx == nullptr) return __ldg(base + (size_t)r * stride);
+  const int32_t* ip = op.idx + (size_t)r * op.width;
+  const float* wp = op.w + (size_t)r * op.width;
+  float v = 0.f;
+  for (int j = 0; j < op.width; ++j) {
+    const int id = __ldg(ip + j);
+    if (id < 0) break;
+    v = fmaf(__ldg(wp + j), __ldg(base + (size_t)id * stride), v);
+  }
+  return v;
+}
+
+// the same for two adjacent columns (base 8-byte aligned, stride even)
+__device__ __forceinline__ float2 pass_row2(const OpView& op, int r, const float* base, size_t stride) {
+  if (op.idx == nullptr) return __ldg(reinterpret_cast<const float2*>(base + (size_t)r * stride));
+  const int32_t* ip = op.idx + (size_t)r * op.width;
+  const float* wp = op.w + (size_t)r * op.width;
+  float2 v = make_float2(0.f, 0.f);
+  for (int j = 0; j < op.width; ++j) {
+    const int id = __ldg(ip + j);
+    if (id < 0) break;
+    const float w = __ldg(wp + j);
+    const float2 s = __ldg(reinterpret_cast<const float2*>(base + (size_t)id * stride));
+    v.x = fmaf(w, s.x, v.x);
+    v.y = fmaf(w, s.y, v.y);
+  }
+  return v;
+}
 
 // all-plain-operand calls (every term an identity operator) on the wgmma kernel (ellconv_tc.cu): 1 = launched, 0 = not eligible
 int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st);

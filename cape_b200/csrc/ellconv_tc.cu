@@ -106,7 +106,9 @@ __device__ __forceinline__ void ell_gather4_pairs(const OpView& op, const int (&
   }
 }
 
-template <int BN, bool DUAL>
+// PASS: the call has pass-through terms (added in the epilogue); a separate instantiation, so that the kernels of the
+// other calls compile exactly as without them
+template <int BN, bool DUAL, bool PASS>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_constant__ ConvParams p, int nqs,
                                                                   int ncol_tiles) {
   using Cfg = ConvCfg<BN, DUAL>;
@@ -314,6 +316,13 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
           v1[0] = fmaf(coef[slot], q[0], v1[0]); v1[1] = fmaf(coef[slot], q[1], v1[1]);
         }
       }
+      if constexpr (PASS) {
+        for (int q = p.nterms; q < p.nterms + p.npass; ++q) {   // pass-through terms (F == ncols)
+          const TermDev& tm = p.terms[q];
+          const float2 s = pass_row2(tm.op, r, tm.src + (size_t)n * tm.src_rows * tm.src_stride + c, (size_t)tm.src_stride);
+          v0[0] += s.x; v0[1] += s.y;
+        }
+      }
       float o1[2], o2[2];
       bool write2 = false;
       if (linear) {
@@ -350,7 +359,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   }
 }
 
-template <int BN, bool DUAL>
+template <int BN, bool DUAL, bool PASS = false>
 int launch_conv(const ConvParams& p, cudaStream_t st) {
   using Cfg = ConvCfg<BN, DUAL>;
   int nqs = 0;
@@ -362,7 +371,7 @@ int launch_conv(const ConvParams& p, cudaStream_t st) {
   const int smem = 1024 + Cfg::RING + BAR_BYTES + nqs * 4;
   static bool configured = false;
   if (!configured) {
-    CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL, PASS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          1024 + Cfg::RING + BAR_BYTES + QS_MAX_FLOATS * 4));
     configured = true;
   }
@@ -373,7 +382,7 @@ int launch_conv(const ConvParams& p, cudaStream_t st) {
     set_error("conv_wg_kernel: too many tiles");
     return -1;
   }
-  conv_wg_kernel<BN, DUAL><<<(unsigned)nblocks, CONV_THREADS, smem, st>>>(p, nqs, ncol_tiles);
+  conv_wg_kernel<BN, DUAL, PASS><<<(unsigned)nblocks, CONV_THREADS, smem, st>>>(p, nqs, ncol_tiles);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;
@@ -413,9 +422,17 @@ int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cu
     if (tm.stash != nullptr && (tm.stash_stride % 4) != 0) return 0;
     kred += tm.F;
   }
+  for (int i = p.nterms; i < p.nterms + p.npass; ++i)   // pass-through terms: float2 loads in the epilogue
+    if (!p.terms[i].vec) return 0;
   if (kred < 64) return 0;                       // tiny reductions: the SIMT kernel is as good and simpler
   const int bn = pick_bn(p.ncols, dual);
   if (!qs_fits(p, bn)) return 0;
+  if (p.npass > 0) {                             // the encoder's residual blocks: single accumulator
+    if (dual) return 0;
+    if (bn == 32) return launch_conv<32, false, true>(p, st);
+    if (bn == 64) return launch_conv<64, false, true>(p, st);
+    return launch_conv<128, false, true>(p, st);
+  }
   if (dual) return bn == 32 ? launch_conv<32, true>(p, st) : launch_conv<64, true>(p, st);
   if (bn == 32) return launch_conv<32, false>(p, st);
   if (bn == 64) return launch_conv<64, false>(p, st);
@@ -426,7 +443,7 @@ int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cu
 int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
   (void)t;
   if (!tensor_cores_enabled() || g_tuning[8] == 1) return 0;
-  if (dual || p.epilogue == CAPE_EPI_AFFINE) return 0;
+  if (dual || p.epilogue == CAPE_EPI_AFFINE || p.npass > 0) return 0;
   if (p.ncols % 16 != 0 || p.ncols < 32 || !p.ovec) return 0;
   if (p.total_rows >= (1LL << 31)) return 0;
   long long kred = 0;

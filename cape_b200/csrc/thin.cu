@@ -401,7 +401,7 @@ __global__ void __launch_bounds__(256) thinout_combine_kernel(const __grid_const
 // returns 1 if launched, 0 if not eligible
 int launch_thin_fwd(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
   (void)t;
-  if (dual || p.epilogue == CAPE_EPI_AFFINE) return 0;
+  if (dual || p.epilogue == CAPE_EPI_AFFINE || p.npass > 0) return 0;   // pass-through terms: ellconv kernels
   if (p.ncols > TH_MAXCOLS || p.ncols < 16) return 0;
   int KF = 0;
   for (int i = 0; i < p.nterms; ++i) {
@@ -460,7 +460,8 @@ int launch_thin_dw(const cape_topology* t, const cape_dw_args* a, const OpView* 
 
 // thin-output conv: 1 = launched (z lives in the topology workspace), 0 = not eligible
 int launch_thinout_fwd(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
-  if (dual || p.epilogue != CAPE_EPI_LINEAR || p.ncols > 4 || p.nterms > TO_MAXT || g_tuning[7] == 1) return 0;
+  if (dual || p.epilogue != CAPE_EPI_LINEAR || p.ncols > 4 || p.nterms > TO_MAXT || p.npass > 0 || g_tuning[7] == 1)
+    return 0;
   const TermDev& t0 = p.terms[0];
   if (!t0.vec || t0.F < 32 || t0.F % 4 != 0 || t0.F > 512) return 0;
   for (int i = 0; i < p.nterms; ++i) {

@@ -179,7 +179,9 @@ class ChebLayer:
     branch) with its backward."""
 
     def __init__(self, net, site, F, C, Fout, W, gW, bias=None, gbias=None, act=ACT_NONE, Wa=None, gWa=None,
-                 bias_per_row=False, need_dx=True, maxN=1, n_cs_slots=1, name=""):
+                 bias_per_row=False, need_dx=True, maxN=1, n_cs_slots=1, name="", fused=False):
+        """fused: always the one-launch forms, so that a caller can add terms of its own to the launch (fwd / bwd
+        `extra`)."""
         self.net, self.tp, self.site, self.name = net, net.tp, site, name
         if (bias is not None or act != ACT_NONE) and not site.pool_is_selection:
             raise NotImplementedError("%s: the down-sampling matrix is not a pure row selection, so pooling cannot be "
@@ -235,6 +237,8 @@ class ChebLayer:
                 self.stash_ga = torch.empty(maxN, site.rows_in, Fout, device=dev)
         self.fwd_mode, self.dx_mode = choose_forms(F, C, Fout, K, site.rows_in, site.rows_out, self.affine, need_dx,
                                                    self.dw_mode, all(o == -1 for o in site.ops), name)
+        if fused:
+            self.fwd_mode, self.dx_mode = "fused", "fused"
         if self.dx_mode == "contract":
             self.Wk, self.Wk_lo = torch.empty(K, F, Fout, device=dev), torch.empty(K, F, Fout, device=dev)
             net.wprep.add(W, F, K, Fout, wk=self.Wk, wk_lo=self.Wk_lo)
@@ -276,7 +280,8 @@ class ChebLayer:
         """The split forms need the tensor-core kernels (they pass K-major weights only)."""
         return E.tensor_cores_enabled(self.tp)
 
-    def fwd(self, x, ycat, out, out2=None):
+    def fwd(self, x, ycat, out, out2=None, extra=()):
+        """extra: more cheb_call terms of the same launch (a layer built with fused=True)."""
         N = x.shape[0]
         s, F, C, K, Fout = self.site, self.F, self.C, self.K, self.Fout
         assert x.shape[1] == s.rows_in and x.shape[2] >= F and out.shape[1] == s.rows_out
@@ -327,14 +332,15 @@ class ChebLayer:
                 if C:
                     t["wc2"] = self.Wa2[F:]
             terms.append(t)
-        cheb_call(self.tp, N, s.rows_out, Fout, terms, out, out2=out2, cond=ycat if C else None,
+        cheb_call(self.tp, N, s.rows_out, Fout, terms + list(extra), out, out2=out2, cond=ycat if C else None,
                   epilogue=EPI_AFFINE if self.affine else EPI_LINEAR, act=self.act, bias=self.bias,
                   bias_per_row=self.bias_per_row, tag=tag)
 
     def bwd(self, x, ycat, g, g_aff=None, dx=None, dx2=None, dx_epi=EPI_LINEAR, dx_aux=None, dx_alpha=E.LEAKY_ALPHA,
-            dycat=None, want_dw=True, cs_slot=0):
+            dycat=None, want_dw=True, cs_slot=0, dx_extra=()):
         """g: gradient w.r.t. the pre-activation of accumulator 0 ([N, rows_out, Fout]);
-        g_aff: gradient w.r.t. the affine branch (= d out) when the layer has one."""
+        g_aff: gradient w.r.t. the affine branch (= d out) when the layer has one;
+        dx_extra: more terms of the data-gradient launch (a layer built with fused=True)."""
         tp, s, F, C, K, Fout = self.tp, self.site, self.F, self.C, self.K, self.Fout
         N = g.shape[0]
         sx = x.shape[2]
@@ -445,7 +451,8 @@ class ChebLayer:
                                      [dict(src=t["src"], op=t["op"], src_rows=s.rows_out, src_stride=Fout)], H,
                                      out_stride=hs, tag=sub("narrow%d" % i))
                         t.update(src=H, op=-1, src_rows=s.rows_in, src_stride=hs)
-                cheb_call(tp, N, s.rows_in, F, terms, dx, out2=dx2, epilogue=dx_epi, aux=dx_aux, alpha=dx_alpha, tag=dtag)
+                cheb_call(tp, N, s.rows_in, F, terms + list(dx_extra), dx, out2=dx2, epilogue=dx_epi, aux=dx_aux,
+                          alpha=dx_alpha, tag=dtag)
             if gs:
                 # dW_k = x^T (op_k^T G): the data-gradient kernel above left op_k^T G in the stash buffers
                 nl = (1 if self.g_merged else K) + (1 if self.affine else 0)
@@ -587,6 +594,80 @@ class GNBlock:
                g_stride=self.Ft)
 
 
+class EncResBlock:
+    """Encoder residual block (res_block, lib/models.py:715-741) at level i:
+        h1 = leaky(cheb_K(x; W1) + b1);   out = D leaky(cheb_K(h1; W2) + skip(x) + b2),
+    skip = x when the channel counts match, else the 1x1 projection x Ws.  The pooling D selects rows, so it is folded
+    into conv2's operators and into the skip.  conv2 and the skip are ONE launch: the projection is one more contracted
+    term, the identity skip a pass-through term (cape_term without weights).  The first block's projection reads the
+    3 coordinates (+ the condition channels), which would drop the fused launch to the fp32 kernel: it runs on the thin
+    kernel into `xs` and enters the launch as a pass-through term.  The data gradient into x is one launch as well:
+    sum_k T_k^T (dh1 W1_k^T) + D^T (g2 Ws^T) or + D^T g2."""
+
+    def __init__(self, net, i, L, D, Fin, C, Fo, K, maxN, order_in=None, order_mid=None, order_out=None):
+        w, g = net._w, net._g
+        tp, dev = net.tp, net.device
+        self.net, self.tp, self.i, self.C, self.Fin, self.Fo = net, tp, i, C, Fin, Fo
+        sc = "generator/encoder/encoder_resblock%d/" % (i + 1)
+        nm = "enc/res%d" % (i + 1)
+        self.conv1 = ChebLayer(net, ConvSite(tp, L, K, order_in=order_in, order_out=order_mid), Fin, C, Fo,
+                               w(sc + "filter_1/weights"), g(sc + "filter_1/weights"), bias=w(sc + "bias_relu_1/bias"),
+                               gbias=g(sc + "bias_relu_1/bias"), act=ACT_LEAKY, need_dx=(i > 0), maxN=maxN,
+                               name=nm + "/conv1", fused=True)
+        self.conv2 = ChebLayer(net, ConvSite(tp, L, K, D=D, order_in=order_mid, order_out=order_out), Fo, 0, Fo,
+                               w(sc + "filter_2/weights"), g(sc + "filter_2/weights"), bias=w(sc + "bias_relu_2/bias"),
+                               gbias=g(sc + "bias_relu_2/bias"), act=ACT_LEAKY, maxN=maxN, name=nm + "/conv2", fused=True)
+        self.skip = ConvSite(tp, L, 1, D=D, order_in=order_in, order_out=order_out)      # x -> D x
+        self.proj = None
+        if (sc + "1x1-conv/weights") in net.specs:
+            self.proj = ChebLayer(net, self.skip, Fin, C, Fo, w(sc + "1x1-conv/weights"), g(sc + "1x1-conv/weights"),
+                                  need_dx=False, maxN=maxN, name=nm + "/1x1")
+        # thin projection (F <= 4 or condition channels): computed apart, added as a pass-through term
+        self.xs = (torch.zeros(maxN, self.skip.rows_out, Fo, device=dev)
+                   if self.proj is not None and (Fin % 4 != 0 or C > 0) else None)
+        self.h1 = torch.zeros(maxN, self.conv1.site.rows_out, Fo, device=dev)
+        self.dh1 = torch.zeros_like(self.h1)
+
+    def layers(self):
+        return [l for l in (self.conv1, self.conv2, self.proj) if l is not None]
+
+    def fwd(self, x, ycat, out):
+        N, sx, sk = x.shape[0], x.shape[2], self.skip
+        h1 = self.h1[:N]
+        self.conv1.fwd(x, ycat, h1)
+        if self.xs is not None:
+            self.proj.fwd(x, ycat, self.xs[:N])
+            t = dict(src=self.xs[:N], op=-1, F=self.Fo, src_rows=sk.rows_out, src_stride=self.Fo, w=None, w_stride=0)
+        elif self.proj is not None:
+            p = self.proj
+            t = dict(src=x, op=sk.ops[0], F=self.Fin, src_rows=sk.rows_in, src_stride=sx, w=p.W3[:, 0, :],
+                     w_stride=self.Fo, wT=p.Wt[0], wT_stride=self.Fin, wT_lo=p.Wt_lo[0])
+            if p.stash_a[0] is not None:
+                t["stash"], t["stash_stride"] = p.stash_a[0][:N], self.Fin
+        else:
+            t = dict(src=x, op=sk.ops[0], F=self.Fin, src_rows=sk.rows_in, src_stride=sx, w=None, w_stride=0)
+        self.conv2.fwd(h1, None, out, extra=[t])
+
+    def bwd(self, x, ycat, g2, dx=None, dx_aux=None, dycat=None):
+        """g2: gradient w.r.t. conv2's pre-activation (the block's output rows); dx (written, SLOPE epilogue with the
+        producing block's output dx_aux) when the block has an input gradient; dycat +=."""
+        N, sk = g2.shape[0], self.skip
+        h1, dh1 = self.h1[:N], self.dh1[:N]
+        self.conv2.bwd(h1, None, g2, dx=dh1, dx_epi=EPI_SLOPE, dx_aux=h1)
+        if self.proj is not None:
+            self.proj.bwd(x, ycat, g2, dycat=dycat)             # weight (and condition) gradients of the projection
+        if dx is None:
+            self.conv1.bwd(x, ycat, dh1, dycat=dycat)
+            return
+        if self.proj is not None:
+            p = self.proj
+            t = dict(src=g2, op=sk.opsT[0], F=self.Fo, src_rows=sk.rows_out, src_stride=self.Fo, w=p.Wt[0],
+                     w_stride=self.Fin, wT=p.W3[:, 0, :], wT_stride=self.Fo, wT_lo=p.W3_lo[:, 0, :])
+        else:
+            t = dict(src=g2, op=sk.opsT[0], F=self.Fo, src_rows=sk.rows_out, src_stride=self.Fo, w=None, w_stride=0)
+        self.conv1.bwd(x, ycat, dh1, dx=dx, dx_epi=EPI_SLOPE, dx_aux=dx_aux, dycat=dycat, dx_extra=[t])
+
+
 class CapeNetwork:
     """Encoder/decoder/discriminator + losses + optimiser on one GPU for a fixed batch size."""
 
@@ -603,9 +684,8 @@ class CapeNetwork:
         self.N = int(batch_size)
         self.ref_compat = bool(ref_compat)
         c = self.cfg
-        if c["use_res_block"] or not c["use_res_block_dec"] or c["cond_encoder"] or c["reduce_dim"] <= 0:
-            raise NotImplementedError("only the shipped-config architecture is built: use_res_block=0, "
-                                      "use_res_block_dec=1, cond_encoder=0, reduce_dim>0")
+        if not c["use_res_block_dec"] or c["reduce_dim"] <= 0:
+            raise NotImplementedError("the plain decoder (use_res_block_dec=0) and reduce_dim=0 are not built")
         if c["optimizer"] not in ("sgd", "adam") or c["loss"] != "l1":
             raise NotImplementedError("optimizer must be 'sgd' (momentum) or 'adam' (lib/models.py:449-453); only "
                                       "loss='l1' is implemented")
@@ -657,13 +737,21 @@ class CapeNetwork:
             og, od = [None] * (nl + 1), [None] * (len(D_d) + 1)
         self.order_g, self.order_d = og, od
         self.enc = []
+        self.enc_res = bool(c["use_res_block"])
+        self.cond_enc = bool(c["cond_encoder"])        # the first encoder layer also sees [y | y2] (models.py:531-535)
         fin = c["nn_input_channel"]
         for i in range(nl):
-            site = ConvSite(tp, L[i], K[i], D=D[i], order_in=og[i] if i > 0 else None, order_out=og[i + 1])
-            sc = "generator/encoder/encoder_conv%d" % (i + 1)
-            self.enc.append(ChebLayer(self, site, fin, 0, F[i], w(sc + "/weights"), g(sc + "/weights"),
-                                      bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=ACT_LEAKY, need_dx=(i > 0),
-                                      maxN=N, name="enc/conv%d" % (i + 1)))
+            Ci = Cc if (self.cond_enc and i == 0) else 0
+            oi = og[i] if i > 0 else None
+            if self.enc_res:
+                self.enc.append(EncResBlock(self, i, L[i], D[i], fin, Ci, F[i], K[i], N, order_in=oi, order_mid=og[i],
+                                            order_out=og[i + 1]))
+            else:
+                site = ConvSite(tp, L[i], K[i], D=D[i], order_in=oi, order_out=og[i + 1])
+                sc = "generator/encoder/encoder_conv%d" % (i + 1)
+                self.enc.append(ChebLayer(self, site, fin, Ci, F[i], w(sc + "/weights"), g(sc + "/weights"),
+                                          bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=ACT_LEAKY, need_dx=(i > 0),
+                                          maxN=N, name="enc/conv%d" % (i + 1)))
             fin = F[i]
         red = specs["generator/encoder/1x1-conv/weights"][1]
         self.red = red
@@ -740,7 +828,8 @@ class CapeNetwork:
         h1 = specs["condition_pose/fc1/dense/kernel"][1]
         self.cp_h = z(2 * N, h1)
         self.cc_h = z(2 * N, specs["condition_clo_label/fc1/dense/kernel"][1]) if self.c_clo2 else None
-        self.enc_act = [z(N, l.site.rows_out, l.Fout) for l in self.enc]
+        enc_shape = [(l.conv2.site.rows_out, l.Fo) if self.enc_res else (l.site.rows_out, l.Fout) for l in self.enc]
+        self.enc_act = [z(N, *s) for s in enc_shape]
         self.enc_red = z(N, self.p[-1], red)
         self.z_mean, self.z_logvar = z(N, nz), z(N, nz)
         self.z_total = z(N, nz + Cc)
@@ -768,7 +857,7 @@ class CapeNetwork:
         self.g_z = z(N, nz)
         self.g_mean, self.g_logvar = z(N, nz), z(N, nz)
         self.g_enc_red = z(N, self.p[-1], red)
-        self.g_enc = [z(N, l.site.rows_out, l.Fout) for l in self.enc]
+        self.g_enc = [z(N, *s) for s in enc_shape]
         self.g_cp_h, self.g_cp_t = z(N, h1), z(N, h1)
         self.g_cc_h = z(N, self.cc_h.shape[1]) if self.c_clo2 else None
         self.g_cc_t = z(N, self.cc_h.shape[1]) if self.c_clo2 else None
@@ -811,7 +900,8 @@ class CapeNetwork:
 
     def all_layers(self):
         dec = self.dec if self.affine else [l for b in self.dec for l in b.layers()]
-        return self.enc + [self.enc_1x1, self.dec_1x1] + dec + [self.dec_out] + self.disc + [self.disc_pred]
+        enc = [l for b in self.enc for l in b.layers()] if self.enc_res else self.enc
+        return enc + [self.enc_1x1, self.dec_1x1] + dec + [self.dec_out] + self.disc + [self.disc_pred]
 
     def run_dw(self, fn):
         """Issue the weight-gradient launches `fn(topology)` of one layer: on the side stream (after everything
@@ -913,9 +1003,10 @@ class CapeNetwork:
 
     def encoder_fwd(self):
         x = self.in_x
+        yc = self.ycat_g if self.cond_enc else None       # the generator batch's condition embeddings
         for l, a in zip(self.enc, self.enc_act):
-            l.fwd(x, None, a)
-            x = a
+            l.fwd(x, yc, a)
+            x, yc = a, None
         self.enc_1x1.fwd(x, None, self.enc_red)
         flat = self.enc_red.view(self.N, self.flat)
         self.fc_mean.fwd(flat, self.z_mean)
@@ -1010,10 +1101,16 @@ class CapeNetwork:
         self._reduce_bucket("enc_fc")                       # 28 MB of gradients are final: all-reduce behind the conv backward
         self.enc_1x1.bwd(self.enc_act[-1], None, self.g_enc_red, dx=self.g_enc[-1], dx_epi=EPI_SLOPE,
                          dx_aux=self.enc_act[-1])
+        yc = self.ycat_g if self.cond_enc else None
+        dyc = self.d_ycat if self.cond_enc else None        # complete before cond_bwd (the small products flush first)
         for i in range(len(self.enc) - 1, 0, -1):
-            self.enc[i].bwd(self.enc_act[i - 1], None, self.g_enc[i], dx=self.g_enc[i - 1], dx_epi=EPI_SLOPE,
-                            dx_aux=self.enc_act[i - 1])
-        self.enc[0].bwd(self.in_x, None, self.g_enc[0])
+            if self.enc_res:
+                self.enc[i].bwd(self.enc_act[i - 1], None, self.g_enc[i], dx=self.g_enc[i - 1],
+                                dx_aux=self.enc_act[i - 1])
+            else:
+                self.enc[i].bwd(self.enc_act[i - 1], None, self.g_enc[i], dx=self.g_enc[i - 1], dx_epi=EPI_SLOPE,
+                                dx_aux=self.enc_act[i - 1])
+        self.enc[0].bwd(self.in_x, yc, self.g_enc[0], dycat=dyc)
 
     def cond_bwd(self):
         """d_ycat (generator batch) -> condition-net weight grads."""

@@ -50,11 +50,20 @@ def param_specs(cfg, p, p_d):
         s["condition_clo_label/fc1/dense/bias"] = (h2,)
         s["condition_clo_label/fc2/dense/kernel"] = (h2, nzc2)
         s["condition_clo_label/fc2/dense/bias"] = (nzc2,)
-    # encoder (models.py:514-561)
-    fin = cfg["nn_input_channel"]
+    # encoder (models.py:514-561); cond_encoder: the first layer also sees [y | y2] on every vertex (:531-535)
+    fin = cfg["nn_input_channel"] + (Cc if cfg.get("cond_encoder") else 0)
     for i in range(len(F)):
-        s["generator/encoder/encoder_conv%d/weights" % (i + 1)] = (fin * K[i], F[i])
-        s["generator/encoder/encoder_conv%d/bias" % (i + 1)] = (1, 1, F[i])
+        if cfg.get("use_res_block"):
+            sc = "generator/encoder/encoder_resblock%d" % (i + 1)        # res_block, models.py:715-741
+            s[sc + "/filter_1/weights"] = (fin * K[i], F[i])
+            s[sc + "/bias_relu_1/bias"] = (1, 1, F[i])
+            s[sc + "/filter_2/weights"] = (F[i] * K[i], F[i])
+            if fin != F[i]:
+                s[sc + "/1x1-conv/weights"] = (fin, F[i])
+            s[sc + "/bias_relu_2/bias"] = (1, 1, F[i])
+        else:
+            s["generator/encoder/encoder_conv%d/weights" % (i + 1)] = (fin * K[i], F[i])
+            s["generator/encoder/encoder_conv%d/bias" % (i + 1)] = (1, 1, F[i])
         fin = F[i]
     rd = cfg["reduce_dim"]
     red = F[-1] // (F[-1] // rd) if rd > 0 else F[-1]

@@ -57,6 +57,10 @@ int cape_topology_reserve_workspace(cape_topology* t, int64_t bytes);
  *   acc0 (and acc1 if w2) += A_t[:, :, :F] @ W_t[:F, :ncols],   W_t element (f, c) = w[f * w_stride + c]
  * plus the condition broadcast without materialising it (lib/models.py:591-594,606-609,663-666):
  *   acc += rowsum(op)[r] * (cond[n, :C] @ Wc_t[:C, :ncols]),    Wc_t element (j, c) = wc[j * w_stride + c]
+ * A term whose w, w2, wT and w2T are all NULL is a PASS-THROUGH term: no contraction,
+ *   acc0 += A_t[:, :, :ncols]      (a residual added before the epilogue's bias / activation / SLOPE mask)
+ * It needs F == ncols and takes no wc, wc2 or stash; a call needs at least one contracted term, and a plain_only call
+ * takes no pass-through term (rc < 0 otherwise).
  */
 typedef struct {
   const float* src;   /* [N, src_rows, src_stride] */

@@ -46,6 +46,9 @@ struct cape_topology {
   std::vector<cape::EllOp> ops;
   void* workspace = nullptr;
   int64_t workspace_bytes = 0;
+  // tile ticket of the persistent conv_wg_kernel (ellconv_tc.cu): device int, zero between launches.  Every launch
+  // that uses it must be ordered after the previous one (one stream, or a graph replayed on one stream).
+  unsigned* tile_counter = nullptr;
 };
 
 namespace cape {

@@ -6,26 +6,32 @@
 // with fp32 accuracy by 3xTF32 error compensation:  a = a_hi + a_lo (a_hi = top 19 bits, a_lo = the exact remainder),
 // acc += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo with fp32 accumulation; the dropped a_lo*b_lo term is ~2^-22 relative.
 //
-// A CTA owns one 128-row x BN-column output tile and runs four warpgroups around a ring of shared-memory stages:
+// The kernel is persistent: one CTA per SM (at most one fits) loops over 128-row x BN-column output tiles (except the
+// instantiations of ConvCfg::ONE_TILE, one tile per CTA), and runs four warpgroups around a ring of shared-memory
+// stages:
 //  - warpgroups 0 and 1, the producers, gather the Chebyshev-basis chunk A[128 rows x 32 k] from neighbour rows
 //    (float4 loads, same ELL tables and row mapping as the SIMT path) or load it from a plain operand, load the weight
 //    chunk B[BN x 32 k] (K-major copy of W), split both into hi/lo and store them in the swizzled K-major layout of the
 //    next free stage, then arrive on the stage's `full` mbarrier;
 //  - warpgroups 2 and 3, the consumers, each own 64 output rows: wait on `full`, issue wgmma m64nBNk8 for the chunk,
-//    wait for it, add the chunk's sum into the running accumulator and release the stage on its `empty` mbarrier.
-// The producers run up to STAGES chunks ahead, so the gather of later chunks overlaps the MMAs of earlier ones, and the
-// two consumers never wait for each other.  setmaxnreg moves registers from the producers to the consumers, which hold
-// the accumulators.  Two producer warpgroups, not one, and each producer thread gathers both of its row pairs at
-// once (16 neighbour-row loads in flight) with the weight chunk's loads issued first: the gather is latency-bound
-// on L2, and fewer loads in flight than the 256-thread lockstep kernel this replaces made the gather-heavy layers
-// slower on the H100.
-// The grid is 1-D with the column tiles fastest, so the CTAs of one row tile run together and read its source rows
-// from L2 rather than from HBM once per column tile.
+//    wait for it, add the chunk's sum into the running accumulator and release the stage on its `empty` mbarrier; at
+//    the tile's last chunk they run the epilogue from the accumulator registers.
+// The producers run up to STAGES chunks ahead, across tile boundaries: the ring's stage and phase run on over the
+// CTA's tiles, so the gather of the next tile overlaps the MMAs and the epilogue of the previous one (most launches
+// of the step have only 2-8 chunks per tile, which a one-tile CTA spends in ramp and drain).  The two consumers never
+// wait for each other.  setmaxnreg moves registers from the producers to the consumers, which hold the accumulators.
+// Two producer warpgroups, not one, and each producer thread gathers both of its row pairs at once (16 neighbour-row
+// loads in flight) with the weight chunk's loads issued first: the gather is latency-bound on L2.
+// Tiles are handed out by ticket (an atomic counter of the topology handle) in the order row tile, then column tile
+// fastest, so the CTAs of one row tile run together and read its source rows from L2 rather than from HBM once per
+// column tile, and a CTA that starts late (the weight-gradient stream holding its SM) simply takes fewer tiles.
 //
 // Every chunk's products go to a fresh register accumulator that is added to the running sum in fp32 with
 // round-to-nearest, so the tensor core's truncating accumulation chain is one chunk (12 MMAs) long instead of the whole
 // reduction: long reductions would otherwise drift from the fp64 truth by more than 1e-4 (cape_conv_args.precise
 // has no effect).
+#include <algorithm>
+#include <type_traits>
 #include "common.cuh"
 #include "ellconv_params.cuh"
 #include "tc_common.cuh"
@@ -46,7 +52,7 @@ constexpr int CONSUMER_REGS = 144;
 constexpr int GATHER_PAIRS = 2;               // row pairs each producer thread gathers at once
 constexpr int A_TILE = BM * 128;              // 128 rows x 32 fp32
 constexpr int QS_MAX_FLOATS = 8192;           // condition vectors of the tile's samples and columns
-constexpr int BAR_BYTES = 256;                // the ring's mbarriers
+constexpr int BAR_BYTES = 256;                // the ring's mbarriers and tile slots
 constexpr int SMEM_MAX = 227 * 1024;          // dynamic shared memory per CTA on sm_90
 
 template <int BN, bool DUAL>
@@ -58,7 +64,11 @@ struct ConvCfg {
   static constexpr int STAGES = FIT < 4 ? FIT : 4;
   static constexpr int RING = STAGES * STAGE;
   static_assert(STAGES >= 3, "the ring needs at least three stages");
-  static_assert(2 * STAGES * 8 <= BAR_BYTES, "mbarrier area too small");
+  static_assert(2 * STAGES * 8 + STAGES * 4 <= BAR_BYTES, "mbarrier area too small");
+  // one tile per CTA (grid = tiles, tile = blockIdx.x, no ticket): the tile loop's state does not fit beside the 16
+  // weight registers of these producers (BN = 128) or the 128 accumulator registers of these consumers (DUAL, BN =
+  // 64), which then spill and run the wide, long-reduction layers that use them slower than one tile per CTA does
+  static constexpr bool ONE_TILE = BN == 128 || (DUAL && BN == 64);
 };
 
 // Gathers rows (ra[i], rb[i]) for NP pairs: the producers' copy of ell_gather4_pair (NP = 1), which this one matches
@@ -107,10 +117,13 @@ __device__ __forceinline__ void ell_gather4_pairs(const OpView& op, const int (&
 }
 
 // PASS: the call has pass-through terms (added in the epilogue); a separate instantiation, so that the kernels of the
-// other calls compile exactly as without them
+// other calls compile exactly as without them.
+// Tiles come from *counter, which is 0 at the start of a launch: each CTA draws tickets until one is past the last
+// tile, so a launch draws exactly ntiles + gridDim.x tickets, and the CTA that draws the last one resets the counter
+// for the next launch of the handle.
 template <int BN, bool DUAL, bool PASS>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_constant__ ConvParams p, int nqs,
-                                                                  int ncol_tiles) {
+                                                                  int ncol_tiles, int ntiles, unsigned* counter) {
   using Cfg = ConvCfg<BN, DUAL>;
   constexpr int S = Cfg::STAGES;
   constexpr int NA = BN / 2;                  // accumulator registers per consumer thread
@@ -118,12 +131,12 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   char* smem = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::RING);
   uint64_t* empty = full + S;
+  // tile_slot[s]: the tile whose first chunk stage s holds (-1: no more tiles), set before the stage's `full` arrive;
+  // one per stage, as the producers run up to a tile ahead of the consumers
+  int* tile_slot = reinterpret_cast<int*>(empty + S);
   float* qs = reinterpret_cast<float*>(smem + Cfg::RING + BAR_BYTES);
 
   const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
-  const int ct = (int)(blockIdx.x % (unsigned)ncol_tiles);
-  const long long row0 = (long long)(blockIdx.x / (unsigned)ncol_tiles) * BM;
-  const int col0 = ct * BN;
 
   // the reduction: 32-deep chunks over all terms (a term of F = 0 still takes one all-zero chunk)
   int nchunks = 0;
@@ -144,223 +157,278 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
     // (rs, rs + 32) and (rs + 64, rs + 96): the row mapping of the SIMT kernels, so each row's taps add in their order
     const int l8 = tid & 7, rs = tid >> 3;
     constexpr int ROWS[4] = {0, 32, 64, 96};
-    int rn[4], rr[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const long long R = row0 + rs + ROWS[i];
-      if (R < p.total_rows) { rn[i] = (int)(R / p.rows_out); rr[i] = (int)(R % p.rows_out); }
-      else { rn[i] = -1; rr[i] = 0; }
-    }
-    const bool do_stash = ct == 0;            // one column tile writes the basis copies
-    int t = 0, f0 = 0;
-    for (int j = 0; j < nchunks; ++j) {
-      const int stage = j % S;
-      mbar_wait(&empty[stage], ((j / S) & 1) ^ 1);
-      char* a_hi = smem + (size_t)stage * Cfg::STAGE;
-      char* a_lo = a_hi + A_TILE;
-      char* b_hi = a_lo + A_TILE;
-      char* b_lo = b_hi + Cfg::B_TILE;
-      const TermDev& tm = p.terms[t];
-      const int f = f0 + l8 * 4;
-      // the weight chunk's loads first: they are independent of the gather and fly while it runs
-      const bool has2 = DUAL && tm.w2T != nullptr;
-      float4 rb[BN / 32], rb2[DUAL ? BN / 32 : 1];
-#pragma unroll
-      for (int i = 0; i < BN / 32; ++i) {
-        const int c = col0 + rs + 32 * i;
-        rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (c < p.ncols && f < tm.F) rb[i] = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
-        if (DUAL) {
-          rb2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (has2 && c < p.ncols && f < tm.F) rb2[i] = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
+    uint32_t it = 0;                          // the CTA's running chunk count: ring stage it % S, phase (it / S) & 1
+    unsigned next = 0;
+    if (!Cfg::ONE_TILE && tid == 0) next = atomicAdd(counter, 1u);
+    for (;;) {
+      int tile = (int)blockIdx.x;
+      if (!Cfg::ONE_TILE) {
+        // the stage of the tile's first chunk takes the tile's index, for the other producers and the consumers
+        mbar_wait(&empty[it % S], ((it / S) & 1) ^ 1);
+        if (tid == 0) tile_slot[it % S] = next < (unsigned)ntiles ? (int)next : -1;
+        named_bar_sync(2, PRODUCER_THREADS);
+        tile = tile_slot[it % S];             // not rewritten before the consumers have released this stage
+        if (tile < 0) {                       // no more tiles
+          if (tid == 0 && next == (unsigned)ntiles + gridDim.x - 1) *counter = 0u;   // the launch's last ticket
+          mbar_arrive(&full[it % S]);
+          return;
         }
+        if (tid == 0) next = atomicAdd(counter, 1u);   // the following tile's ticket, in flight during this tile
       }
+      const int ct = tile % ncol_tiles;
+      const long long row0 = (long long)(tile / ncol_tiles) * BM;
+      const int col0 = ct * BN;
+      int rn[4], rr[4];
 #pragma unroll
-      for (int h = 0; h < 2 / GATHER_PAIRS; ++h) {  // GATHER_PAIRS pairs (ROWS[2q], ROWS[2q + 1]) at a time
-        constexpr int NP = GATHER_PAIRS;
-        float4 va[NP], vb[NP];
+      for (int i = 0; i < 4; ++i) {
+        const long long R = row0 + rs + ROWS[i];
+        if (R < p.total_rows) { rn[i] = (int)(R / p.rows_out); rr[i] = (int)(R % p.rows_out); }
+        else { rn[i] = -1; rr[i] = 0; }
+      }
+      const bool do_stash = ct == 0;          // one column tile writes the basis copies
+      int t = 0, f0 = 0;
+      for (int j = 0; j < nchunks; ++j, ++it) {
+        const int stage = it % S;
+        mbar_wait(&empty[stage], ((it / S) & 1) ^ 1);
+        char* a_hi = smem + (size_t)stage * Cfg::STAGE;
+        char* a_lo = a_hi + A_TILE;
+        char* b_hi = a_lo + A_TILE;
+        char* b_lo = b_hi + Cfg::B_TILE;
+        const TermDev& tm = p.terms[t];
+        const int f = f0 + l8 * 4;
+        // the weight chunk's loads first: they are independent of the gather and fly while it runs
+        const bool has2 = DUAL && tm.w2T != nullptr;
+        float4 rb[BN / 32], rb2[DUAL ? BN / 32 : 1];
 #pragma unroll
-        for (int q = 0; q < NP; ++q) { va[q] = make_float4(0.f, 0.f, 0.f, 0.f); vb[q] = va[q]; }
-        if (f < tm.F) {
-          // invalid (beyond-the-end) rows gather sample 0 / row 0 and are zeroed afterwards
-          const float* base_a[NP];
-          const float* base_b[NP];
-          int ra[NP], rb_[NP];
-#pragma unroll
-          for (int q = 0; q < NP; ++q) {
-            const int ia = 2 * (h * NP + q);
-            base_a[q] = tm.src + (size_t)max(rn[ia], 0) * tm.src_rows * tm.src_stride + f;
-            base_b[q] = tm.src + (size_t)max(rn[ia + 1], 0) * tm.src_rows * tm.src_stride + f;
-            ra[q] = rr[ia]; rb_[q] = rr[ia + 1];
+        for (int i = 0; i < BN / 32; ++i) {
+          const int c = col0 + rs + 32 * i;
+          rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+          if (c < p.ncols && f < tm.F) rb[i] = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
+          if (DUAL) {
+            rb2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (has2 && c < p.ncols && f < tm.F) rb2[i] = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
           }
-          if (tm.op.idx == nullptr) {
+        }
+#pragma unroll
+        for (int h = 0; h < 2 / GATHER_PAIRS; ++h) {  // GATHER_PAIRS pairs (ROWS[2q], ROWS[2q + 1]) at a time
+          constexpr int NP = GATHER_PAIRS;
+          float4 va[NP], vb[NP];
+#pragma unroll
+          for (int q = 0; q < NP; ++q) { va[q] = make_float4(0.f, 0.f, 0.f, 0.f); vb[q] = va[q]; }
+          if (f < tm.F) {
+            // invalid (beyond-the-end) rows gather sample 0 / row 0 and are zeroed afterwards
+            const float* base_a[NP];
+            const float* base_b[NP];
+            int ra[NP], rb_[NP];
 #pragma unroll
             for (int q = 0; q < NP; ++q) {
-              va[q] = ldg4(base_a[q] + (size_t)ra[q] * tm.src_stride);
-              vb[q] = ldg4(base_b[q] + (size_t)rb_[q] * tm.src_stride);
+              const int ia = 2 * (h * NP + q);
+              base_a[q] = tm.src + (size_t)max(rn[ia], 0) * tm.src_rows * tm.src_stride + f;
+              base_b[q] = tm.src + (size_t)max(rn[ia + 1], 0) * tm.src_rows * tm.src_stride + f;
+              ra[q] = rr[ia]; rb_[q] = rr[ia + 1];
             }
-          } else {
-            ell_gather4_pairs<NP>(tm.op, ra, rb_, base_a, base_b, (size_t)tm.src_stride, va, vb);
+            if (tm.op.idx == nullptr) {
+#pragma unroll
+              for (int q = 0; q < NP; ++q) {
+                va[q] = ldg4(base_a[q] + (size_t)ra[q] * tm.src_stride);
+                vb[q] = ldg4(base_b[q] + (size_t)rb_[q] * tm.src_stride);
+              }
+            } else {
+              ell_gather4_pairs<NP>(tm.op, ra, rb_, base_a, base_b, (size_t)tm.src_stride, va, vb);
+            }
+          }
+#pragma unroll
+          for (int q = 0; q < NP; ++q) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int i = 2 * (h * NP + q) + e;
+              float4 v = e == 0 ? va[q] : vb[q];
+              if (rn[i] < 0) v = make_float4(0.f, 0.f, 0.f, 0.f);
+              const int row = rs + ROWS[i];
+              if (f < tm.F && tm.stash != nullptr && do_stash && rn[i] >= 0)   // basis rows for the weight gradient
+                *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row) * tm.stash_stride + f) = v;
+              split_store4(v, a_hi, a_lo, (uint32_t)(row * 128 + ((l8 ^ (row & 7)) << 4)));
+            }
           }
         }
 #pragma unroll
-        for (int q = 0; q < NP; ++q) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int i = 2 * (h * NP + q) + e;
-            float4 v = e == 0 ? va[q] : vb[q];
-            if (rn[i] < 0) v = make_float4(0.f, 0.f, 0.f, 0.f);
-            const int row = rs + ROWS[i];
-            if (f < tm.F && tm.stash != nullptr && do_stash && rn[i] >= 0)   // basis rows for the weight gradient
-              *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row) * tm.stash_stride + f) = v;
-            split_store4(v, a_hi, a_lo, (uint32_t)(row * 128 + ((l8 ^ (row & 7)) << 4)));
-          }
+        for (int i = 0; i < BN / 32; ++i) {
+          const int cl = rs + 32 * i;
+          const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
+          split_store4(rb[i], b_hi, b_lo, off);
+          if (DUAL) split_store4(rb2[i], b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, off);
         }
+        fence_proxy_async();                  // generic-proxy smem writes -> visible to the tensor core's (async) proxy
+        mbar_arrive(&full[stage]);
+        f0 += BK;
+        if (f0 >= tm.F) { f0 = 0; ++t; }
       }
-#pragma unroll
-      for (int i = 0; i < BN / 32; ++i) {
-        const int cl = rs + 32 * i;
-        const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
-        split_store4(rb[i], b_hi, b_lo, off);
-        if (DUAL) split_store4(rb2[i], b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, off);
-      }
-      fence_proxy_async();                    // generic-proxy smem writes -> visible to the tensor core's (async) proxy
-      mbar_arrive(&full[stage]);
-      f0 += BK;
-      if (f0 >= tm.F) { f0 = 0; ++t; }
+      if (Cfg::ONE_TILE) return;
     }
-    return;
   }
 
   // =========================== consumers ===========================
   setmaxnreg_inc<CONSUMER_REGS>();
   const int cw = wg - 2, ctid = tid - PRODUCER_THREADS;
-
-  // condition broadcast vectors of this tile: qs[s][slot][c] = cond[n_first + s, :] . Wc_slot[:, col0 + c]
-  const int n_first = (int)(row0 / p.rows_out);
-  if (p.nslots > 0) {
-    for (int o = ctid; o < nqs; o += CONSUMER_THREADS) {
-      const int c = o % BN, slot = (o / BN) % p.nslots, s = o / (BN * p.nslots);
-      float q = 0.f;
-      const int n = n_first + s;
-      if (col0 + c < p.ncols && n < p.N) {
-        const float* y = p.cond + (size_t)n * p.C;
-        const float* wc = p.slot_w[slot] + col0 + c;
-        const int ws = p.slot_acc[slot] ? p.terms[p.slot_term[slot]].w2_stride : p.terms[p.slot_term[slot]].w_stride;
-        for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * ws), q);
-      }
-      qs[o] = q;
-    }
-  }
-
-  float acc0[NA], acc1[DUAL ? NA : 1], part0[NA], part1[DUAL ? NA : 1];
-#pragma unroll
-  for (int i = 0; i < NA; ++i) { acc0[i] = 0.f; if (DUAL) acc1[i] = 0.f; }
-
-  for (int j = 0; j < nchunks; ++j) {
-    const int stage = j % S;
-    mbar_wait(&full[stage], (j / S) & 1);
-    const uint32_t a_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + (uint32_t)(cw * 64 * 128);
-    const uint32_t a_lo = a_hi + A_TILE;
-    const uint32_t b_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + 2 * A_TILE;
-    const uint32_t b_lo = b_hi + Cfg::B_TILE;
-    wgmma_fence();
-    fence_acc(part0);
-    mma3_chunk<BN>(part0, a_hi, a_lo, b_hi, b_lo, 0);
-    if constexpr (DUAL) {
-      fence_acc(part1);
-      mma3_chunk<BN>(part1, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
-    }
-    wgmma_commit();
-    wgmma_wait_all();
-    if ((tid & 31) == 0) mbar_arrive(&empty[stage]);   // this warp's MMAs have read the stage
-    fence_acc(part0);
-#pragma unroll
-    for (int i = 0; i < NA; ++i) acc0[i] += part0[i];
-    if constexpr (DUAL) {
-      fence_acc(part1);
-#pragma unroll
-      for (int i = 0; i < NA; ++i) acc1[i] += part1[i];
-    }
-  }
-  named_bar_sync(1, CONSUMER_THREADS);        // qs complete (written before the main loop, read below)
-
-  // =========================== epilogue: straight from the accumulator registers ===========================
   const bool linear = p.epilogue == CAPE_EPI_LINEAR;
   const bool use_aux = p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {                       // the thread's two rows
-    const int lrow = cw * 64 + frag_row(wt, 2 * h);
-    const long long R = row0 + lrow;
-    if (R >= p.total_rows) continue;
-    const int n = (int)(R / p.rows_out), r = (int)(R % p.rows_out);
-    const size_t orow = (size_t)R * p.ncols;
-    float coef[MAX_SLOTS];
-    for (int slot = 0; slot < p.nslots; ++slot) {
-      const TermDev& tm = p.terms[p.slot_term[slot]];
-      coef[slot] = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
+  uint32_t it = 0;                            // as the producers' count
+  for (;;) {
+    int tile = (int)blockIdx.x;
+    if (!Cfg::ONE_TILE) {
+      mbar_wait(&full[it % S], (it / S) & 1); // the tile's first chunk carries its index
+      tile = tile_slot[it % S];
+      if (tile < 0) return;
     }
-    const float* bias_row = (linear && p.bias != nullptr) ? p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) : nullptr;
+
+    float acc0[NA], acc1[DUAL ? NA : 1], part0[NA], part1[DUAL ? NA : 1];
 #pragma unroll
-    for (int g = 0; g < NA / 4; ++g) {
-      const int i = 4 * g + 2 * h;
-      const int c = col0 + frag_col(wt, i);
-      if (c >= p.ncols) continue;
-      float v0[2] = {acc0[i], acc0[i + 1]}, v1[2] = {0.f, 0.f};
-      if (DUAL) { v1[0] = acc1[i]; v1[1] = acc1[i + 1]; }
+    for (int i = 0; i < NA; ++i) { acc0[i] = 0.f; if (DUAL) acc1[i] = 0.f; }
+
+    for (const uint32_t end = it + nchunks; it != end; ++it) {
+      const int stage = it % S;
+      mbar_wait(&full[stage], (it / S) & 1);
+      const uint32_t a_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + (uint32_t)(cw * 64 * 128);
+      const uint32_t a_lo = a_hi + A_TILE;
+      const uint32_t b_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + 2 * A_TILE;
+      const uint32_t b_lo = b_hi + Cfg::B_TILE;
+      wgmma_fence();
+      fence_acc(part0);
+      mma3_chunk<BN>(part0, a_hi, a_lo, b_hi, b_lo, 0);
+      if constexpr (DUAL) {
+        fence_acc(part1);
+        mma3_chunk<BN>(part1, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
+      }
+      wgmma_commit();
+      wgmma_wait_all();
+      if ((tid & 31) == 0) mbar_arrive(&empty[stage]);   // this warp's MMAs have read the stage (and its tile slot)
+      fence_acc(part0);
+#pragma unroll
+      for (int i = 0; i < NA; ++i) acc0[i] += part0[i];
+      if constexpr (DUAL) {
+        fence_acc(part1);
+#pragma unroll
+        for (int i = 0; i < NA; ++i) acc1[i] += part1[i];
+      }
+    }
+
+    // the tile's coordinates only now, so that they take no registers beside the accumulators in the loop above
+    const int ct = tile % ncol_tiles;
+    const long long row0 = (long long)(tile / ncol_tiles) * BM;
+    const int col0 = ct * BN;
+    // condition broadcast vectors of this tile: qs[s][slot][c] = cond[n_first + s, :] . Wc_slot[:, col0 + c]
+    const int n_first = (int)(row0 / p.rows_out);
+    if (p.nslots > 0) {
+      named_bar_sync(1, CONSUMER_THREADS);    // the previous tile's epilogue has read qs
+      for (int o = ctid; o < nqs; o += CONSUMER_THREADS) {
+        const int c = o % BN, slot = (o / BN) % p.nslots, s = o / (BN * p.nslots);
+        float q = 0.f;
+        const int n = n_first + s;
+        if (col0 + c < p.ncols && n < p.N) {
+          const float* y = p.cond + (size_t)n * p.C;
+          const float* wc = p.slot_w[slot] + col0 + c;
+          const int ws = p.slot_acc[slot] ? p.terms[p.slot_term[slot]].w2_stride : p.terms[p.slot_term[slot]].w_stride;
+          for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * ws), q);
+        }
+        qs[o] = q;
+      }
+      named_bar_sync(1, CONSUMER_THREADS);    // qs complete
+    }
+
+    // =========================== epilogue: straight from the accumulator registers ===========================
+    // the thread's two rows, h = 0 and 1, each as its own copy of the code: with a loop over h, the accumulators of a
+    // wide tile could end up indexed at run time (in local memory)
+    auto row_epilogue = [&](auto h_const) {
+      constexpr int h = decltype(h_const)::value;
+      const int lrow = cw * 64 + frag_row(wt, 2 * h);
+      const long long R = row0 + lrow;
+      if (R >= p.total_rows) return;
+      const int n = (int)(R / p.rows_out), r = (int)(R % p.rows_out);
+      const size_t orow = (size_t)R * p.ncols;
+      // condition slots, then pass-through terms, into the accumulators in place: each slot or term is a runtime loop
+      // around the unrolled columns, so that the accumulators are only ever indexed by constants
       for (int slot = 0; slot < p.nslots; ++slot) {
-        const float* q = qs + ((size_t)(n - n_first) * p.nslots + slot) * BN + (c - col0);
+        const TermDev& tm = p.terms[p.slot_term[slot]];
+        const float coef = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
+        const float* q = qs + ((size_t)(n - n_first) * p.nslots + slot) * BN + frag_col(wt, 0);
         if (p.slot_acc[slot] == 0) {
-          v0[0] = fmaf(coef[slot], q[0], v0[0]); v0[1] = fmaf(coef[slot], q[1], v0[1]);
+#pragma unroll
+          for (int g = 0; g < NA / 4; ++g) {
+            const int i = 4 * g + 2 * h;
+            acc0[i] = fmaf(coef, q[8 * g], acc0[i]); acc0[i + 1] = fmaf(coef, q[8 * g + 1], acc0[i + 1]);
+          }
         } else if (DUAL) {
-          v1[0] = fmaf(coef[slot], q[0], v1[0]); v1[1] = fmaf(coef[slot], q[1], v1[1]);
+#pragma unroll
+          for (int g = 0; g < NA / 4; ++g) {
+            const int i = 4 * g + 2 * h;
+            acc1[i] = fmaf(coef, q[8 * g], acc1[i]); acc1[i + 1] = fmaf(coef, q[8 * g + 1], acc1[i + 1]);
+          }
         }
       }
       if constexpr (PASS) {
         for (int q = p.nterms; q < p.nterms + p.npass; ++q) {   // pass-through terms (F == ncols)
           const TermDev& tm = p.terms[q];
-          const float2 s = pass_row2(tm.op, r, tm.src + (size_t)n * tm.src_rows * tm.src_stride + c, (size_t)tm.src_stride);
-          v0[0] += s.x; v0[1] += s.y;
+          const float* src = tm.src + (size_t)n * tm.src_rows * tm.src_stride;
+#pragma unroll
+          for (int g = 0; g < NA / 4; ++g) {
+            const int i = 4 * g + 2 * h;
+            const int c = col0 + frag_col(wt, i);
+            if (c >= p.ncols) continue;
+            const float2 s = pass_row2(tm.op, r, src + c, (size_t)tm.src_stride);
+            acc0[i] += s.x; acc0[i + 1] += s.y;
+          }
         }
       }
-      float o1[2], o2[2];
-      bool write2 = false;
-      if (linear) {
+      const float* bias_row = (linear && p.bias != nullptr) ? p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) : nullptr;
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          float v = v0[e] + (bias_row != nullptr ? __ldg(bias_row + c + e) : 0.f);
-          if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
-          else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
-          o1[e] = v;
-        }
-      } else if (p.epilogue == CAPE_EPI_AFFINE) {
-        write2 = p.out2 != nullptr;
+      for (int g = 0; g < NA / 4; ++g) {
+        const int i = 4 * g + 2 * h;
+        const int c = col0 + frag_col(wt, i);
+        if (c >= p.ncols) continue;
+        float v0[2] = {acc0[i], acc0[i + 1]}, v1[2] = {0.f, 0.f};
+        if (DUAL) { v1[0] = acc1[i]; v1[1] = acc1[i + 1]; }
+        float o1[2], o2[2];
+        bool write2 = false;
+        if (linear) {
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float rg = fmaxf(v0[e], 0.f);
-          o1[e] = (DUAL ? v1[e] : 0.f) + rg;
-          o2[e] = rg;
-        }
-      } else {
-        const float2 ax = use_aux ? __ldg(reinterpret_cast<const float2*>(p.aux + orow + c)) : make_float2(0.f, 0.f);
-        const float a2[2] = {ax.x, ax.y};
-        if (p.epilogue == CAPE_EPI_SLOPE) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) o1[e] = v0[e] * (a2[e] > 0.f ? 1.f : p.alpha);
-        } else {
+          for (int e = 0; e < 2; ++e) {
+            float v = v0[e] + (bias_row != nullptr ? __ldg(bias_row + c + e) : 0.f);
+            if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
+            else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
+            o1[e] = v;
+          }
+        } else if (p.epilogue == CAPE_EPI_AFFINE) {
           write2 = p.out2 != nullptr;
 #pragma unroll
-          for (int e = 0; e < 2; ++e) { o1[e] = v0[e]; o2[e] = a2[e] > 0.f ? v0[e] : 0.f; }
+          for (int e = 0; e < 2; ++e) {
+            const float rg = fmaxf(v0[e], 0.f);
+            o1[e] = (DUAL ? v1[e] : 0.f) + rg;
+            o2[e] = rg;
+          }
+        } else {
+          const float2 ax = use_aux ? __ldg(reinterpret_cast<const float2*>(p.aux + orow + c)) : make_float2(0.f, 0.f);
+          const float a2[2] = {ax.x, ax.y};
+          if (p.epilogue == CAPE_EPI_SLOPE) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) o1[e] = v0[e] * (a2[e] > 0.f ? 1.f : p.alpha);
+          } else {
+            write2 = p.out2 != nullptr;
+#pragma unroll
+            for (int e = 0; e < 2; ++e) { o1[e] = v0[e]; o2[e] = a2[e] > 0.f ? v0[e] : 0.f; }
+          }
         }
+        *reinterpret_cast<float2*>(p.out + orow + c) = make_float2(o1[0], o1[1]);
+        if (write2) *reinterpret_cast<float2*>(p.out2 + orow + c) = make_float2(o2[0], o2[1]);
       }
-      *reinterpret_cast<float2*>(p.out + orow + c) = make_float2(o1[0], o1[1]);
-      if (write2) *reinterpret_cast<float2*>(p.out2 + orow + c) = make_float2(o2[0], o2[1]);
-    }
+    };
+    row_epilogue(std::integral_constant<int, 0>{});
+    row_epilogue(std::integral_constant<int, 1>{});
+    if (Cfg::ONE_TILE) return;
   }
 }
 
 template <int BN, bool DUAL, bool PASS = false>
-int launch_conv(const ConvParams& p, cudaStream_t st) {
+int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
   using Cfg = ConvCfg<BN, DUAL>;
   int nqs = 0;
   if (p.nslots > 0) {
@@ -375,14 +443,15 @@ int launch_conv(const ConvParams& p, cudaStream_t st) {
                                          1024 + Cfg::RING + BAR_BYTES + QS_MAX_FLOATS * 4));
     configured = true;
   }
-  // 1-D grid, column tiles fastest (no 65,535 limit on the row tiles)
+  // tiles numbered with the column tiles fastest; one persistent CTA per SM (or per tile, if fewer)
   const int ncol_tiles = (p.ncols + BN - 1) / BN;
-  const long long nblocks = (p.total_rows + BM - 1) / BM * ncol_tiles;
-  if (nblocks >= (1LL << 31)) {
+  const long long ntiles = (p.total_rows + BM - 1) / BM * ncol_tiles;
+  if (ntiles + t->sm_count >= (1LL << 31)) {
     set_error("conv_wg_kernel: too many tiles");
     return -1;
   }
-  conv_wg_kernel<BN, DUAL, PASS><<<(unsigned)nblocks, CONV_THREADS, smem, st>>>(p, nqs, ncol_tiles);
+  const int grid = Cfg::ONE_TILE ? (int)ntiles : (int)std::min<long long>(ntiles, t->sm_count);
+  conv_wg_kernel<BN, DUAL, PASS><<<grid, CONV_THREADS, smem, st>>>(p, nqs, ncol_tiles, (int)ntiles, t->tile_counter);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;
@@ -410,7 +479,6 @@ int g_tuning[32] = {0};   // experiment knobs (cape_set_tuning), see ellconv_par
 bool tensor_cores_enabled() { return g_tc_enabled; }
 
 int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
-  (void)t;
   if (!g_tc_enabled) return 0;
   if (p.ncols % 32 != 0 || p.ncols < 32 || !p.ovec) return 0;
   if ((dual ? 2 : 1) * p.ncols > 512) return 0;
@@ -429,19 +497,18 @@ int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cu
   if (!qs_fits(p, bn)) return 0;
   if (p.npass > 0) {                             // the encoder's residual blocks: single accumulator
     if (dual) return 0;
-    if (bn == 32) return launch_conv<32, false, true>(p, st);
-    if (bn == 64) return launch_conv<64, false, true>(p, st);
-    return launch_conv<128, false, true>(p, st);
+    if (bn == 32) return launch_conv<32, false, true>(t, p, st);
+    if (bn == 64) return launch_conv<64, false, true>(t, p, st);
+    return launch_conv<128, false, true>(t, p, st);
   }
-  if (dual) return bn == 32 ? launch_conv<32, true>(p, st) : launch_conv<64, true>(p, st);
-  if (bn == 32) return launch_conv<32, false>(p, st);
-  if (bn == 64) return launch_conv<64, false>(p, st);
-  return launch_conv<128, false>(p, st);
+  if (dual) return bn == 32 ? launch_conv<32, true>(t, p, st) : launch_conv<64, true>(t, p, st);
+  if (bn == 32) return launch_conv<32, false>(t, p, st);
+  if (bn == 64) return launch_conv<64, false>(t, p, st);
+  return launch_conv<128, false>(t, p, st);
 }
 
 // all-plain-operand calls: 1 = launched, 0 = not eligible (the caller falls through to the gather kernels)
 int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
-  (void)t;
   if (!tensor_cores_enabled() || g_tuning[8] == 1) return 0;
   if (dual || p.epilogue == CAPE_EPI_AFFINE || p.npass > 0) return 0;
   if (p.ncols % 16 != 0 || p.ncols < 32 || !p.ovec) return 0;
@@ -458,9 +525,9 @@ int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaS
     if (p.slot_acc[s] != 0) return 0;
   const int bn = pick_bn(p.ncols, false);
   if (!qs_fits(p, bn)) return 0;
-  if (bn == 32) return launch_conv<32, false>(p, st);
-  if (bn == 64) return launch_conv<64, false>(p, st);
-  return launch_conv<128, false>(p, st);
+  if (bn == 32) return launch_conv<32, false>(t, p, st);
+  if (bn == 64) return launch_conv<64, false>(t, p, st);
+  return launch_conv<128, false>(t, p, st);
 }
 
 }  // namespace cape

@@ -29,6 +29,13 @@ extern "C" int cape_topology_create(int device, cape_topology** out) {
   cudaDeviceProp prop;
   CAPE_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
   t->sm_count = prop.multiProcessorCount;
+  if (cudaMalloc(&t->tile_counter, sizeof(unsigned)) != cudaSuccess ||
+      cudaMemset(t->tile_counter, 0, sizeof(unsigned)) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
+    set_error("cape_topology_create: tile counter allocation failed");
+    cudaFree(t->tile_counter);
+    delete t;
+    return -2;
+  }
   *out = t;
   return 0;
 }
@@ -42,6 +49,7 @@ extern "C" void cape_topology_destroy(cape_topology* t) {
     cudaFree(o.rowsum);
   }
   if (t->workspace) cudaFree(t->workspace);
+  cudaFree(t->tile_counter);
   delete t;
 }
 

@@ -6,13 +6,14 @@
 // with fp32 accuracy by 3xTF32 error compensation:  a = a_hi + a_lo (a_hi = top 19 bits, a_lo = the exact remainder),
 // acc += a_hi*b_hi + a_lo*b_hi + a_hi*b_lo with fp32 accumulation; the dropped a_lo*b_lo term is ~2^-22 relative.
 //
-// The kernel is persistent: one CTA per SM (at most one fits) loops over 128-row x BN-column output tiles (except the
-// instantiations of ConvCfg::ONE_TILE, one tile per CTA), and runs four warpgroups around a ring of shared-memory
-// stages:
+// The kernel is persistent: one CTA per SM (at most one fits) loops over 128-row x BN-column output tiles, and runs
+// four warpgroups around a ring of shared-memory stages:
 //  - warpgroups 0 and 1, the producers, gather the Chebyshev-basis chunk A[128 rows x 32 k] from neighbour rows
-//    (float4 loads, same ELL tables and row mapping as the SIMT path) or load it from a plain operand, load the weight
-//    chunk B[BN x 32 k] (K-major copy of W), split both into hi/lo and store them in the swizzled K-major layout of the
-//    next free stage, then arrive on the stage's `full` mbarrier;
+//    (float4 loads, same ELL tables and row mapping as the SIMT path) or load it from a plain operand, split it into
+//    hi/lo and store it in the swizzled K-major layout of the next free stage.  The weight chunk B[BN x 32 k] (K-major
+//    copy of W) comes by TMA, issued by one producer before the gather, straight into the stage's hi tile in the same
+//    layout; after the gather the producers split it in place into hi/lo.  Then they arrive on the stage's `full`
+//    mbarrier;
 //  - warpgroups 2 and 3, the consumers, each own 64 output rows: wait on `full`, issue wgmma m64nBNk8 for the chunk,
 //    wait for it, add the chunk's sum into the running accumulator and release the stage on its `empty` mbarrier; at
 //    the tile's last chunk they run the epilogue from the accumulator registers.
@@ -21,7 +22,7 @@
 // of the step have only 2-8 chunks per tile, which a one-tile CTA spends in ramp and drain).  The two consumers never
 // wait for each other.  setmaxnreg moves registers from the producers to the consumers, which hold the accumulators.
 // Two producer warpgroups, not one, and each producer thread gathers both of its row pairs at once (16 neighbour-row
-// loads in flight) with the weight chunk's loads issued first: the gather is latency-bound on L2.
+// loads in flight): the gather is latency-bound on L2.  The weights take no producer registers while it runs.
 // Tiles are handed out by ticket (an atomic counter of the topology handle) in the order row tile, then column tile
 // fastest, so the CTAs of one row tile run together and read its source rows from L2 rather than from HBM once per
 // column tile, and a CTA that starts late (the weight-gradient stream holding its SM) simply takes fewer tiles.
@@ -30,7 +31,10 @@
 // round-to-nearest, so the tensor core's truncating accumulation chain is one chunk (12 MMAs) long instead of the whole
 // reduction: long reductions would otherwise drift from the fp64 truth by more than 1e-4 (cape_conv_args.precise
 // has no effect).
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <algorithm>
+#include <cstring>
 #include <type_traits>
 #include "common.cuh"
 #include "ellconv_params.cuh"
@@ -64,11 +68,14 @@ struct ConvCfg {
   static constexpr int STAGES = FIT < 4 ? FIT : 4;
   static constexpr int RING = STAGES * STAGE;
   static_assert(STAGES >= 3, "the ring needs at least three stages");
-  static_assert(2 * STAGES * 8 + STAGES * 4 <= BAR_BYTES, "mbarrier area too small");
-  // one tile per CTA (grid = tiles, tile = blockIdx.x, no ticket): the tile loop's state does not fit beside the 16
-  // weight registers of these producers (BN = 128) or the 128 accumulator registers of these consumers (DUAL, BN =
-  // 64), which then spill and run the wide, long-reduction layers that use them slower than one tile per CTA does
-  static constexpr bool ONE_TILE = BN == 128 || (DUAL && BN == 64);
+  static_assert(3 * STAGES * 8 + STAGES * 4 <= BAR_BYTES, "mbarrier area too small");
+};
+
+// TMA descriptors of the terms' K-major weight copies, encoded at launch: w[t][0] maps wT and w[t][1] w2T of term t,
+// each as a [ncols x F] tensor (row stride wT_stride) read in boxes of 32 k x BN columns with the 128-byte swizzle,
+// the layout of the stage's weight tiles; the zero fill beyond F and ncols pads the last chunk and column tile
+struct WeightMaps {
+  CUtensorMap w[CAPE_MAX_TERMS][2];
 };
 
 // Gathers rows (ra[i], rb[i]) for NP pairs: the producers' copy of ell_gather4_pair (NP = 1), which this one matches
@@ -122,7 +129,8 @@ __device__ __forceinline__ void ell_gather4_pairs(const OpView& op, const int (&
 // tile, so a launch draws exactly ntiles + gridDim.x tickets, and the CTA that draws the last one resets the counter
 // for the next launch of the handle.
 template <int BN, bool DUAL, bool PASS>
-__global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_constant__ ConvParams p, int nqs,
+__global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_constant__ ConvParams p,
+                                                                  const __grid_constant__ WeightMaps maps, int nqs,
                                                                   int ncol_tiles, int ntiles, unsigned* counter) {
   using Cfg = ConvCfg<BN, DUAL>;
   constexpr int S = Cfg::STAGES;
@@ -131,9 +139,10 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   char* smem = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::RING);
   uint64_t* empty = full + S;
+  uint64_t* wfull = empty + S;                // the stage's weight tiles have landed (TMA transaction bytes)
   // tile_slot[s]: the tile whose first chunk stage s holds (-1: no more tiles), set before the stage's `full` arrive;
   // one per stage, as the producers run up to a tile ahead of the consumers
-  int* tile_slot = reinterpret_cast<int*>(empty + S);
+  int* tile_slot = reinterpret_cast<int*>(wfull + S);
   float* qs = reinterpret_cast<float*>(smem + Cfg::RING + BAR_BYTES);
 
   const int tid = threadIdx.x, wg = tid >> 7, wt = tid & 127;
@@ -146,7 +155,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
     for (int s = 0; s < S; ++s) {
       mbar_init(&full[s], PRODUCER_THREADS);  // every producer thread
       mbar_init(&empty[s], 8);                // one lane per consumer warp
+      mbar_init(&wfull[s], 1);                // the producer that issues the stage's weight loads
     }
+    fence_mbar_init();
   }
   __syncthreads();
 
@@ -159,22 +170,19 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
     constexpr int ROWS[4] = {0, 32, 64, 96};
     uint32_t it = 0;                          // the CTA's running chunk count: ring stage it % S, phase (it / S) & 1
     unsigned next = 0;
-    if (!Cfg::ONE_TILE && tid == 0) next = atomicAdd(counter, 1u);
+    if (tid == 0) next = atomicAdd(counter, 1u);
     for (;;) {
-      int tile = (int)blockIdx.x;
-      if (!Cfg::ONE_TILE) {
-        // the stage of the tile's first chunk takes the tile's index, for the other producers and the consumers
-        mbar_wait(&empty[it % S], ((it / S) & 1) ^ 1);
-        if (tid == 0) tile_slot[it % S] = next < (unsigned)ntiles ? (int)next : -1;
-        named_bar_sync(2, PRODUCER_THREADS);
-        tile = tile_slot[it % S];             // not rewritten before the consumers have released this stage
-        if (tile < 0) {                       // no more tiles
-          if (tid == 0 && next == (unsigned)ntiles + gridDim.x - 1) *counter = 0u;   // the launch's last ticket
-          mbar_arrive(&full[it % S]);
-          return;
-        }
-        if (tid == 0) next = atomicAdd(counter, 1u);   // the following tile's ticket, in flight during this tile
+      // the stage of the tile's first chunk takes the tile's index, for the other producers and the consumers
+      mbar_wait(&empty[it % S], ((it / S) & 1) ^ 1);
+      if (tid == 0) tile_slot[it % S] = next < (unsigned)ntiles ? (int)next : -1;
+      named_bar_sync(2, PRODUCER_THREADS);
+      const int tile = tile_slot[it % S];     // not rewritten before the consumers have released this stage
+      if (tile < 0) {                         // no more tiles
+        if (tid == 0 && next == (unsigned)ntiles + gridDim.x - 1) *counter = 0u;   // the launch's last ticket
+        mbar_arrive(&full[it % S]);
+        return;
       }
+      if (tid == 0) next = atomicAdd(counter, 1u);   // the following tile's ticket, in flight during this tile
       const int ct = tile % ncol_tiles;
       const long long row0 = (long long)(tile / ncol_tiles) * BM;
       const int col0 = ct * BN;
@@ -196,18 +204,12 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
         char* b_lo = b_hi + Cfg::B_TILE;
         const TermDev& tm = p.terms[t];
         const int f = f0 + l8 * 4;
-        // the weight chunk's loads first: they are independent of the gather and fly while it runs
+        // the weight chunk first, by TMA into the hi tiles: it lands while the gather runs
         const bool has2 = DUAL && tm.w2T != nullptr;
-        float4 rb[BN / 32], rb2[DUAL ? BN / 32 : 1];
-#pragma unroll
-        for (int i = 0; i < BN / 32; ++i) {
-          const int c = col0 + rs + 32 * i;
-          rb[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (c < p.ncols && f < tm.F) rb[i] = ldg4(tm.wT + (size_t)c * tm.wT_stride + f);
-          if (DUAL) {
-            rb2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (has2 && c < p.ncols && f < tm.F) rb2[i] = ldg4(tm.w2T + (size_t)c * tm.w2T_stride + f);
-          }
+        if (tid == 0) {
+          mbar_arrive_expect_tx(&wfull[stage], (has2 ? 2 : 1) * Cfg::B_TILE);
+          tma_load_2d(b_hi, &maps.w[t][0], f0, col0, &wfull[stage]);
+          if (has2) tma_load_2d(b_lo + Cfg::B_TILE, &maps.w[t][1], f0, col0, &wfull[stage]);
         }
 #pragma unroll
         for (int h = 0; h < 2 / GATHER_PAIRS; ++h) {  // GATHER_PAIRS pairs (ROWS[2q], ROWS[2q + 1]) at a time
@@ -251,19 +253,24 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
             }
           }
         }
+        // the weight chunk, split in place: hi = tf32_hi(w), lo = w - hi (zeros for a term without w2T)
+        mbar_wait(&wfull[stage], (it / S) & 1);
 #pragma unroll
         for (int i = 0; i < BN / 32; ++i) {
           const int cl = rs + 32 * i;
           const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
-          split_store4(rb[i], b_hi, b_lo, off);
-          if (DUAL) split_store4(rb2[i], b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, off);
+          split_store4(*reinterpret_cast<const float4*>(b_hi + off), b_hi, b_lo, off);
+          if (DUAL) {
+            char* b2_hi = b_lo + Cfg::B_TILE;
+            const float4 v2 = has2 ? *reinterpret_cast<const float4*>(b2_hi + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+            split_store4(v2, b2_hi, b2_hi + Cfg::B_TILE, off);
+          }
         }
         fence_proxy_async();                  // generic-proxy smem writes -> visible to the tensor core's (async) proxy
         mbar_arrive(&full[stage]);
         f0 += BK;
         if (f0 >= tm.F) { f0 = 0; ++t; }
       }
-      if (Cfg::ONE_TILE) return;
     }
   }
 
@@ -274,14 +281,14 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   const bool use_aux = p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK;
   uint32_t it = 0;                            // as the producers' count
   for (;;) {
-    int tile = (int)blockIdx.x;
-    if (!Cfg::ONE_TILE) {
-      mbar_wait(&full[it % S], (it / S) & 1); // the tile's first chunk carries its index
-      tile = tile_slot[it % S];
-      if (tile < 0) return;
-    }
+    mbar_wait(&full[it % S], (it / S) & 1);   // the tile's first chunk carries its index
+    const int tile = tile_slot[it % S];
+    if (tile < 0) return;
 
-    float acc0[NA], acc1[DUAL ? NA : 1], part0[NA], part1[DUAL ? NA : 1];
+    // one chunk accumulator for both running sums where two would not fit beside them (DUAL, BN = 64): the second
+    // sum's MMAs then wait for the first one's add
+    constexpr bool ONE_PART = DUAL && BN == 64;
+    float acc0[NA], acc1[DUAL ? NA : 1], part0[NA], part1[DUAL && !ONE_PART ? NA : 1];
 #pragma unroll
     for (int i = 0; i < NA; ++i) { acc0[i] = 0.f; if (DUAL) acc1[i] = 0.f; }
 
@@ -295,17 +302,27 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
       wgmma_fence();
       fence_acc(part0);
       mma3_chunk<BN>(part0, a_hi, a_lo, b_hi, b_lo, 0);
-      if constexpr (DUAL) {
+      if constexpr (DUAL && !ONE_PART) {
         fence_acc(part1);
         mma3_chunk<BN>(part1, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
       }
       wgmma_commit();
       wgmma_wait_all();
+      if constexpr (ONE_PART) {
+        fence_acc(part0);
+#pragma unroll
+        for (int i = 0; i < NA; ++i) acc0[i] += part0[i];
+        wgmma_fence();
+        fence_acc(part0);
+        mma3_chunk<BN>(part0, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
+        wgmma_commit();
+        wgmma_wait_all();
+      }
       if ((tid & 31) == 0) mbar_arrive(&empty[stage]);   // this warp's MMAs have read the stage (and its tile slot)
       fence_acc(part0);
 #pragma unroll
-      for (int i = 0; i < NA; ++i) acc0[i] += part0[i];
-      if constexpr (DUAL) {
+      for (int i = 0; i < NA; ++i) (ONE_PART ? acc1 : acc0)[i] += part0[i];
+      if constexpr (DUAL && !ONE_PART) {
         fence_acc(part1);
 #pragma unroll
         for (int i = 0; i < NA; ++i) acc1[i] += part1[i];
@@ -423,13 +440,55 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
     };
     row_epilogue(std::integral_constant<int, 0>{});
     row_epilogue(std::integral_constant<int, 1>{});
-    if (Cfg::ONE_TILE) return;
   }
+}
+
+// cuTensorMapEncodeTiled from the driver the runtime has loaded (the library does not link against libcuda)
+PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
+  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
+  if (fn == nullptr) {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &f, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
+  }
+  return fn;
+}
+
+// wT (row c at wT + c * stride, F valid k) as a [ncols x F] tensor in boxes of 32 k x BN columns
+int encode_weight_map(CUtensorMap* m, const float* wT, int F, int stride, int ncols, int bn) {
+  const auto encode = tensor_map_encoder();
+  if (encode == nullptr) {
+    set_error("conv_wg_kernel: cuTensorMapEncodeTiled is not available from the CUDA driver");
+    return -2;
+  }
+  const cuuint64_t dims[2] = {(cuuint64_t)F, (cuuint64_t)ncols};
+  const cuuint64_t strides[1] = {(cuuint64_t)stride * sizeof(float)};
+  const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)bn};
+  const cuuint32_t estrides[2] = {1, 1};
+  const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(wT), dims, strides, box, estrides,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("conv_wg_kernel: cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
+    return -2;
+  }
+  return 0;
 }
 
 template <int BN, bool DUAL, bool PASS = false>
 int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
   using Cfg = ConvCfg<BN, DUAL>;
+  WeightMaps maps;
+  memset(&maps, 0, sizeof(maps));
+  for (int i = 0; i < p.nterms; ++i) {
+    const TermDev& tm = p.terms[i];
+    if (encode_weight_map(&maps.w[i][0], tm.wT, tm.F, tm.wT_stride, p.ncols, BN) != 0) return -2;
+    if (DUAL && tm.w2T != nullptr &&
+        encode_weight_map(&maps.w[i][1], tm.w2T, tm.F, tm.w2T_stride, p.ncols, BN) != 0)
+      return -2;
+  }
   int nqs = 0;
   if (p.nslots > 0) {
     const long long rlast_max = BM - 1;
@@ -450,8 +509,9 @@ int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
     set_error("conv_wg_kernel: too many tiles");
     return -1;
   }
-  const int grid = Cfg::ONE_TILE ? (int)ntiles : (int)std::min<long long>(ntiles, t->sm_count);
-  conv_wg_kernel<BN, DUAL, PASS><<<grid, CONV_THREADS, smem, st>>>(p, nqs, ncol_tiles, (int)ntiles, t->tile_counter);
+  const int grid = (int)std::min<long long>(ntiles, t->sm_count);
+  conv_wg_kernel<BN, DUAL, PASS><<<grid, CONV_THREADS, smem, st>>>(p, maps, nqs, ncol_tiles, (int)ntiles,
+                                                                   t->tile_counter);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;

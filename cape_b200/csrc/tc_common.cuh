@@ -33,12 +33,25 @@ __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// shared-memory mbarriers (thread arrivals only, no transaction counts) for producer/consumer rings
+// shared-memory mbarriers for producer/consumer rings: thread arrivals, and the transaction bytes of TMA loads
 __device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
 }
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
+// makes the initialised mbarriers visible to the asynchronous proxy (TMA completions), before the __syncthreads
+__device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// arrives and adds `bytes` to the transaction count the phase waits for (issued before the loads that complete them)
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+// TMA: the box at coordinates (x0 innermost, x1) of a 2-d tensor map into shared memory (`dst` 1024-byte aligned for
+// the 128-byte swizzle), completing its bytes on `bar`; elements outside the tensor are filled with zeros
+__device__ __forceinline__ void tma_load_2d(void* dst, const void* tmap, int x0, int x1, uint64_t* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(x0), "r"(x1), "r"(smem_u32(bar)) : "memory");
 }
 // waits until the phase of parity `parity` has completed (a fresh barrier counts its phase "before 0" as parity 1)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {

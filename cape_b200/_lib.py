@@ -18,15 +18,14 @@ class Term(C.Structure):
     _fields_ = [("src", C.c_void_p), ("op", C.c_int), ("F", C.c_int), ("src_rows", C.c_int),
                 ("src_stride", C.c_int), ("w_stride", C.c_int), ("w2_stride", C.c_int), ("w", C.c_void_p), ("w2", C.c_void_p),
                 ("wc", C.c_void_p), ("wc2", C.c_void_p), ("wT", C.c_void_p), ("w2T", C.c_void_p),
-                ("wT_stride", C.c_int), ("w2T_stride", C.c_int), ("stash", C.c_void_p), ("stash_stride", C.c_int),
-                ("wT_lo", C.c_void_p), ("w2T_lo", C.c_void_p)]
+                ("wT_stride", C.c_int), ("w2T_stride", C.c_int), ("stash", C.c_void_p), ("stash_stride", C.c_int)]
 
 
 class ConvArgs(C.Structure):
     _fields_ = [("N", C.c_int), ("rows_out", C.c_int), ("ncols", C.c_int), ("nterms", C.c_int),
                 ("terms", Term * MAX_TERMS), ("cond", C.c_void_p), ("C", C.c_int), ("epilogue", C.c_int),
                 ("act", C.c_int), ("alpha", C.c_float), ("bias", C.c_void_p), ("bias_per_row", C.c_int),
-                ("aux", C.c_void_p), ("out", C.c_void_p), ("out2", C.c_void_p), ("precise", C.c_int), ("plain_only", C.c_int)]
+                ("aux", C.c_void_p), ("out", C.c_void_p), ("out2", C.c_void_p), ("plain_only", C.c_int)]
 
 
 class ApplyTerm(C.Structure):
@@ -44,7 +43,7 @@ class ApplyArgs(C.Structure):
 
 class WPrep(C.Structure):
     _fields_ = [("w", C.c_void_p), ("Fin", C.c_int), ("K", C.c_int), ("Fout", C.c_int), ("wt", C.c_void_p),
-                ("wt_lo", C.c_void_p), ("wk", C.c_void_p), ("wk_lo", C.c_void_p)]
+                ("wk", C.c_void_p)]
 
 
 class GemmItem(C.Structure):
@@ -86,8 +85,7 @@ SIGNATURES = {
                             C.c_float, C.c_void_p]),
     "cape_resample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                 C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
-    "cape_cheb_weight_transpose": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "cape_tf32_lo": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "cape_cheb_weight_transpose": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "cape_act_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_void_p]),
     "cape_axpy": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_int64, C.c_void_p]),
     "cape_vae_sample_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,

@@ -714,7 +714,6 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
     d.wT = s.wT; d.w2T = s.w2T; d.wT_stride = s.wT_stride; d.w2T_stride = s.w2T_stride;
     d.vec = (s.F % 4 == 0) && (s.src_stride % 4 == 0) && aligned16(s.src);
     d.stash = s.stash; d.stash_stride = s.stash_stride;
-    d.wT_lo = s.wT_lo; d.w2T_lo = s.w2T_lo;
     if (s.stash) {
       CAPE_REQUIRE(s.F % 4 == 0 && s.stash_stride >= s.F && s.stash_stride % 4 == 0 && aligned16(s.stash),
                    "stash needs F % 4 == 0, stash_stride % 4 == 0 and 16-byte alignment");

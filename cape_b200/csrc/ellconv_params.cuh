@@ -20,8 +20,6 @@ struct TermDev {
   const float* w2T;
   int wT_stride, w2T_stride;
   int vec;
-  const float* wT_lo;   // optional: wT - trunc_tf32(wT), same layout (not read by the wgmma kernels)
-  const float* w2T_lo;
   float* stash;       // optional copy of the gathered basis rows [total_rows, stash_stride] (cape_term.stash)
   int stash_stride;
 };
@@ -43,7 +41,6 @@ struct ConvParams {
   int bias_per_row;
   // terms[0, nterms) are contracted; terms[nterms, nterms + npass) are pass-through terms (cape_term with no weights:
   // acc0 += op . src[:, :, :ncols] in the epilogue).  A launcher that does not add them must decline a call with npass > 0.
-  // (Here it fills the padding before `aux`: the layout of the other fields is unchanged.)
   int npass;
   const float* aux;
   float* out;

@@ -29,8 +29,7 @@
 //
 // Every chunk's products go to a fresh register accumulator that is added to the running sum in fp32 with
 // round-to-nearest, so the tensor core's truncating accumulation chain is one chunk (12 MMAs) long instead of the whole
-// reduction: long reductions would otherwise drift from the fp64 truth by more than 1e-4 (cape_conv_args.precise
-// has no effect).
+// reduction: long reductions would otherwise drift from the fp64 truth by more than 1e-4.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <algorithm>
@@ -593,7 +592,7 @@ int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaS
 }  // namespace cape
 
 extern "C" int cape_set_tuning(int key, int value) {
-  if (key < 0 || key >= 32) return -1;
+  CAPE_REQUIRE(key == 7 || key == 8 || key == 10 || key == 16 || key == 17, "unknown tuning key");
   const int prev = cape::g_tuning[key];
   cape::g_tuning[key] = value;
   return prev;

@@ -216,8 +216,7 @@ __global__ void adam_kernel(float* __restrict__ w, const float* __restrict__ g, 
   }
 }
 
-__global__ void wtrans_kernel(const float* __restrict__ w, int Fin, int K, int Fout, float* __restrict__ wt,
-                              float* __restrict__ wt_lo) {
+__global__ void wtrans_kernel(const float* __restrict__ w, int Fin, int K, int Fout, float* __restrict__ wt) {
   // tile transpose through shared memory: for each k, [Fin x Fout] -> [Fout x Fin]
   __shared__ float tile[32][33];
   const int k = blockIdx.z;
@@ -229,11 +228,7 @@ __global__ void wtrans_kernel(const float* __restrict__ w, int Fin, int K, int F
   __syncthreads();
   for (int i = threadIdx.y; i < 32; i += blockDim.y) {
     const int c = c0 + i, f = f0 + threadIdx.x;
-    if (c < Fout && f < Fin) {
-      const float v = tile[threadIdx.x][i];
-      wt[((size_t)c * K + k) * Fin + f] = v;
-      if (wt_lo) wt_lo[((size_t)c * K + k) * Fin + f] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-    }
+    if (c < Fout && f < Fin) wt[((size_t)c * K + k) * Fin + f] = tile[threadIdx.x][i];
   }
 }
 
@@ -271,31 +266,15 @@ __global__ void __launch_bounds__(256) wprep_kernel(const cape_wprep* __restrict
       const int f = f0 + i, c = c0 + tx;
       const float v = (f < d.Fin && c < d.Fout) ? d.w[((size_t)f * d.K + k) * d.Fout + c] : 0.f;
       tile[i][tx] = v;
-      if (d.wk != nullptr && f < d.Fin && c < d.Fout) {
-        const size_t o = ((size_t)k * d.Fin + f) * d.Fout + c;
-        d.wk[o] = v;
-        if (d.wk_lo != nullptr) d.wk_lo[o] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-      }
+      if (d.wk != nullptr && f < d.Fin && c < d.Fout) d.wk[((size_t)k * d.Fin + f) * d.Fout + c] = v;
     }
     __syncthreads();
     if (d.wt != nullptr) {
       for (int i = ty; i < 32; i += 8) {
         const int c = c0 + i, f = f0 + tx;
-        if (c < d.Fout && f < d.Fin) {
-          const float v = tile[tx][i];
-          const size_t o = ((size_t)k * d.Fout + c) * d.Fin + f;
-          d.wt[o] = v;
-          if (d.wt_lo != nullptr) d.wt_lo[o] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
-        }
+        if (c < d.Fout && f < d.Fin) d.wt[((size_t)k * d.Fout + c) * d.Fin + f] = tile[tx][i];
       }
     }
-  }
-}
-
-__global__ void tf32_lo_kernel(const float* __restrict__ x, float* __restrict__ lo, long long n) {
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float v = x[i];
-    lo[i] = v - __uint_as_float(__float_as_uint(v) & 0xffffe000u);
   }
 }
 
@@ -416,11 +395,10 @@ extern "C" int cape_adam_clip_update(float* w, const float* g, float* m, float* 
   return 0;
 }
 
-extern "C" int cape_cheb_weight_transpose(const float* w, int Fin, int K, int Fout, float* wt, float* wt_lo,
-                                          void* stream) {
+extern "C" int cape_cheb_weight_transpose(const float* w, int Fin, int K, int Fout, float* wt, void* stream) {
   CAPE_REQUIRE(w && wt && Fin > 0 && K > 0 && Fout > 0, "bad arguments");
   dim3 grid((Fin + 31) / 32, (Fout + 31) / 32, K), block(32, 8);
-  wtrans_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(w, Fin, K, Fout, wt, wt_lo);
+  wtrans_kernel<<<grid, block, 0, (cudaStream_t)stream>>>(w, Fin, K, Fout, wt);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   return 0;
@@ -445,14 +423,6 @@ extern "C" int cape_weight_prep(const cape_wprep* descs_device, int n, int block
   if (blocks_per_desc < 1) blocks_per_desc = 8;
   dim3 grid((unsigned)blocks_per_desc, (unsigned)n);
   wprep_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(descs_device);
-  CAPE_CHECK_CUDA(cudaGetLastError());
-  cape::count_launches(1);
-  return 0;
-}
-
-extern "C" int cape_tf32_lo(const float* x, float* lo, long long n, void* stream) {
-  CAPE_REQUIRE(x && lo && n > 0, "bad arguments");
-  tf32_lo_kernel<<<blocks_for(n, 256, 4096), 256, 0, (cudaStream_t)stream>>>(x, lo, n);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   return 0;

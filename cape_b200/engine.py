@@ -145,12 +145,11 @@ def gemm(tp, A, B, Cout, bias=None, act=ACT_NONE, alpha=1.0, beta=0.0, tag=None)
 
 
 def cheb_call(tp, N, rows_out, ncols, terms, out, out2=None, cond=None, epilogue=EPI_LINEAR, act=ACT_NONE,
-              alpha=LEAKY_ALPHA, bias=None, bias_per_row=False, aux=None, tag=None, precise=False, plain_only=False,
-              family="ellconv"):
+              alpha=LEAKY_ALPHA, bias=None, bias_per_row=False, aux=None, tag=None, plain_only=False, family="ellconv"):
     """terms: list of dicts(src, op, F, src_rows, src_stride, w, w_stride, w2, wc, wc2) with torch tensors.
-    precise / plain_only: cape_conv_args fields of the same names (short accumulation chains; TMA-fed kernel or error)."""
+    plain_only: the cape_conv_args field of the same name (TMA-fed kernel or error)."""
     a = ConvArgs()
-    a.precise, a.plain_only = (1 if precise else 0), (1 if plain_only else 0)
+    a.plain_only = 1 if plain_only else 0
     a.N, a.rows_out, a.ncols, a.nterms = N, rows_out, ncols, len(terms)
     for i, t in enumerate(terms):
         d = a.terms[i]
@@ -162,7 +161,7 @@ def cheb_call(tp, N, rows_out, ncols, terms, out, out2=None, cond=None, epilogue
         d.w_stride = t["w_stride"]
         d.w2_stride = t.get("w2_stride", 0)
         d.w = t["w"].data_ptr() if t.get("w") is not None else None
-        for k in ("w2", "wc", "wc2", "wT", "w2T", "stash", "wT_lo", "w2T_lo"):
+        for k in ("w2", "wc", "wc2", "wT", "w2T", "stash"):
             v = t.get(k)
             setattr(d, k, v.data_ptr() if v is not None else None)
         d.wT_stride = t.get("wT_stride", 0)
@@ -225,17 +224,17 @@ class WeightPrep:
         self.tp, self.items, self.table = tp, [], None
         self.blocks_per_desc = int(__import__("os").environ.get("CAPE_WPREP_BLOCKS", "128"))
 
-    def add(self, w, Fin, K, Fout, wt=None, wt_lo=None, wk=None, wk_lo=None):
-        self.items.append((w, Fin, K, Fout, wt, wt_lo, wk, wk_lo))
+    def add(self, w, Fin, K, Fout, wt=None, wk=None):
+        self.items.append((w, Fin, K, Fout, wt, wk))
 
     def run(self):
         if not self.items:
             return
         if self.table is None:
             arr = (WPrep * len(self.items))()
-            for d, (w, Fin, K, Fout, wt, wt_lo, wk, wk_lo) in zip(arr, self.items):
+            for d, (w, Fin, K, Fout, wt, wk) in zip(arr, self.items):
                 d.w, d.Fin, d.K, d.Fout = w.data_ptr(), Fin, K, Fout
-                for nm, t in (("wt", wt), ("wt_lo", wt_lo), ("wk", wk), ("wk_lo", wk_lo)):
+                for nm, t in (("wt", wt), ("wk", wk)):
                     setattr(d, nm, t.data_ptr() if t is not None else None)
             raw = np.frombuffer(bytes(arr), dtype=np.uint8).copy()
             self.table = torch.from_numpy(raw).to(self.tp.device)
@@ -325,13 +324,8 @@ def colsum(tp, g, N, rows, ncols, ops, out, g_stride=None):
                              _ptr(out), _stream()))
 
 
-def weight_transpose(tp, w, Fin, K, Fout, wt, wt_lo=None):
-    check(tp.lib.cape_cheb_weight_transpose(_ptr(w), Fin, K, Fout, _ptr(wt), _ptr(wt_lo), _stream()))
-
-
-def tf32_lo(tp, x, lo):
-    """lo = x - tf32_trunc(x) (the pre-split low part of an operand the tensor cores read raw)."""
-    check(tp.lib.cape_tf32_lo(_ptr(_f32(x)), _ptr(_f32(lo)), x.numel(), _stream()))
+def weight_transpose(tp, w, Fin, K, Fout, wt):
+    check(tp.lib.cape_cheb_weight_transpose(_ptr(w), Fin, K, Fout, _ptr(wt), _stream()))
 
 
 def act_bwd(tp, dy, y, g, alpha=LEAKY_ALPHA):

@@ -46,19 +46,11 @@ class ParamStore:
         self.flat = torch.zeros(self.size, device=device)
         self.grad = torch.zeros(self.size, device=device)
         self.mom = torch.zeros(self.size, device=device)
-        self.lo = torch.zeros(self.size, device=device)     # flat - tf32_trunc(flat): cape_term.wT_lo (unread by the wgmma kernels)
         self.var = None                                     # Adam's second-moment slot (`mom` is its first): add_adam_slot()
 
     def add_adam_slot(self):
         if self.var is None:
             self.var = torch.zeros(self.size, device=self.flat.device)
-
-    def lo_of(self, t):
-        """The view of `lo` that corresponds to `t`, a contiguous view of `flat`; None if t is not one."""
-        off = (t.data_ptr() - self.flat.data_ptr()) // 4
-        if t.data_ptr() < self.flat.data_ptr() or off + t.numel() > self.size or not t.is_contiguous():
-            return None
-        return self.lo[off: off + t.numel()].view(t.shape)
 
     def _view(self, buf, n):
         k = int(np.prod(self.shapes[n]))
@@ -203,12 +195,10 @@ class ChebLayer:
         #      contract-first forward Z = X @ [W_0 | W_1 | ... | W_a];
         #   Wk [K, F, Fout]: per-order plain copies, B operand of the contract-first data gradient Z = G @ [W_k^T]_k.
         A = 1 if self.affine else 0
-        self.Wt, self.Wt_lo = torch.empty(K + A, Fout, F, device=dev), torch.empty(K + A, Fout, F, device=dev)
-        self.W3_lo = net.lo_of(W).view(F + C, K, Fout)
-        net.wprep.add(W, F, K, Fout, wt=self.Wt[:K], wt_lo=self.Wt_lo[:K])
+        self.Wt = torch.empty(K + A, Fout, F, device=dev)
+        net.wprep.add(W, F, K, Fout, wt=self.Wt[:K])
         if self.affine:
-            self.Wa2_lo = net.lo_of(Wa).view(F + C, Fout)
-            net.wprep.add(Wa, F, 1, Fout, wt=self.Wt[K:], wt_lo=self.Wt_lo[K:])
+            net.wprep.add(Wa, F, 1, Fout, wt=self.Wt[K:])
         # Where the weight gradient gets its operands (all three end in the same contraction  dW = A^T G over rows):
         #   "aside":  the forward kernel also writes the gathered basis B_k = op_k x (cape_term.stash), dW_k = B_k^T G;
         #   "gside":  the data-gradient kernel also writes H_k = op_k^T G, dW_k = x^T H_k -- all K terms in ONE pass
@@ -240,8 +230,8 @@ class ChebLayer:
         if fused:
             self.fwd_mode, self.dx_mode = "fused", "fused"
         if self.dx_mode == "contract":
-            self.Wk, self.Wk_lo = torch.empty(K, F, Fout, device=dev), torch.empty(K, F, Fout, device=dev)
-            net.wprep.add(W, F, K, Fout, wk=self.Wk, wk_lo=self.Wk_lo)
+            self.Wk = torch.empty(K, F, Fout, device=dev)
+            net.wprep.add(W, F, K, Fout, wk=self.Wk)
             net.scratch_req(maxN * site.rows_out * K * F)
         if self.fwd_mode == "contract":
             net.scratch_req(maxN * site.rows_in * (K + A) * Fout)
@@ -294,7 +284,7 @@ class ChebLayer:
             Z = self.net.scratch[: N * s.rows_in * ncz].view(N, s.rows_in, ncz)
             cheb_call(self.tp, N, s.rows_in, ncz,
                       [dict(src=x, op=-1, F=F, src_rows=s.rows_in, src_stride=sx, w=None, w_stride=0,
-                            wT=self.Wt.view(ncz, F), wT_stride=F, wT_lo=self.Wt_lo.view(ncz, F))],
+                            wT=self.Wt.view(ncz, F), wT_stride=F)],
                       Z, plain_only=True, tag=sub("project"))
             terms = [dict(src=Z[:, :, k * Fout:], op=s.ops[k], src_rows=s.rows_in, src_stride=ncz, acc=0,
                           wc=self.W3[F:, k, :] if C else None, wc_stride=K * Fout) for k in range(K)]
@@ -319,7 +309,7 @@ class ChebLayer:
         terms = []
         for k in range(K):
             t = dict(src=x, op=s.ops[k], F=F, src_rows=s.rows_in, src_stride=sx, w=self.W3[:, k, :],
-                     w_stride=K * Fout, wT=self.Wt[k], wT_stride=F, wT_lo=self.Wt_lo[k])
+                     w_stride=K * Fout, wT=self.Wt[k], wT_stride=F)
             if C:
                 t["wc"] = self.W3[F:, k, :]
             if basis and s.ops[k] != -1:
@@ -328,7 +318,7 @@ class ChebLayer:
                 t["stash"], t["stash_stride"] = self.stash_a[k][:N], F
             if self.affine and k == 0:
                 t["w2"], t["w2_stride"] = self.Wa2, Fout
-                t["w2T"], t["w2T_stride"], t["w2T_lo"] = self.Wt[K], F, self.Wt_lo[K]
+                t["w2T"], t["w2T_stride"] = self.Wt[K], F
                 if C:
                     t["wc2"] = self.Wa2[F:]
             terms.append(t)
@@ -420,7 +410,7 @@ class ChebLayer:
                 Z = self.net.scratch[: N * s.rows_out * K * F].view(N, s.rows_out, K * F)
                 cheb_call(tp, N, s.rows_out, K * F,
                           [dict(src=g, op=-1, F=Fout, src_rows=s.rows_out, src_stride=Fout, w=None, w_stride=0,
-                                wT=self.Wk.view(K * F, Fout), wT_stride=Fout, wT_lo=self.Wk_lo.view(K * F, Fout))],
+                                wT=self.Wk.view(K * F, Fout), wT_stride=Fout)],
                           Z, plain_only=True, tag=sub("project"))
                 E.apply_call(tp, N, s.rows_in, F,
                              [dict(src=Z[:, :, k * F:], op=s.opsT[k], src_rows=s.rows_out, src_stride=K * F)
@@ -430,14 +420,13 @@ class ChebLayer:
                 terms = []
                 if self.affine:
                     t = dict(src=g_aff, op=s.opsT[0], F=Fout, src_rows=s.rows_out, src_stride=Fout, w=self.Wt[K],
-                             w_stride=F, wT=self.Wa2, wT_stride=Fout, wT_lo=self.Wa2_lo)
+                             w_stride=F, wT=self.Wa2, wT_stride=Fout)
                     if gs and self.stash_ga is not None:
                         t["stash"], t["stash_stride"] = self.stash_ga[:N], Fout
                     terms.append(t)
                 for k in range(K):
                     t = dict(src=g, op=s.opsT[k], F=Fout, src_rows=s.rows_out, src_stride=Fout,
-                             w=self.Wt[k], w_stride=F, wT=self.W3[:, k, :], wT_stride=K * Fout,
-                             wT_lo=self.W3_lo[:, k, :])
+                             w=self.Wt[k], w_stride=F, wT=self.W3[:, k, :], wT_stride=K * Fout)
                     if gs and self.stash_g[k] is not None:
                         t["stash"], t["stash_stride"] = self.stash_g[k][:N], self.stash_g[k].stride(1)
                     terms.append(t)
@@ -563,10 +552,10 @@ class GNBlock:
         E.gn_relu_fwd(tp, self.H2, g2["gamma"], g2["beta"], self.A3, g2["stats"], g2["G"])
         l2, li = self.lin2, self.lin_in
         terms = [dict(src=self.A3, op=-1, F=self.mid, src_rows=self.rows, src_stride=self.mid, w=l2.W3[:, 0, :],
-                      w_stride=self.Fo, wT=l2.Wt[0], wT_stride=self.mid, wT_lo=l2.Wt_lo[0])]
+                      w_stride=self.Fo, wT=l2.Wt[0], wT_stride=self.mid)]
         if li is not None:
             terms.append(dict(src=self.Z, op=-1, F=self.Ft, src_rows=self.rows, src_stride=self.Ft, w=li.W3[:, 0, :],
-                              w_stride=self.Fo, wT=li.Wt[0], wT_stride=self.Ft, wT_lo=li.Wt_lo[0]))
+                              w_stride=self.Fo, wT=li.Wt[0], wT_stride=self.Ft))
         cheb_call(tp, N, self.rows, self.Fo, terms, out,
                   tag=("dec/res:out", l2.alg_bytes(N, "fwd") + (li.alg_bytes(N, "fwd") if li is not None else 0)))
         if li is None:
@@ -641,7 +630,7 @@ class EncResBlock:
         elif self.proj is not None:
             p = self.proj
             t = dict(src=x, op=sk.ops[0], F=self.Fin, src_rows=sk.rows_in, src_stride=sx, w=p.W3[:, 0, :],
-                     w_stride=self.Fo, wT=p.Wt[0], wT_stride=self.Fin, wT_lo=p.Wt_lo[0])
+                     w_stride=self.Fo, wT=p.Wt[0], wT_stride=self.Fin)
             if p.stash_a[0] is not None:
                 t["stash"], t["stash_stride"] = p.stash_a[0][:N], self.Fin
         else:
@@ -662,7 +651,7 @@ class EncResBlock:
         if self.proj is not None:
             p = self.proj
             t = dict(src=g2, op=sk.opsT[0], F=self.Fo, src_rows=sk.rows_out, src_stride=self.Fo, w=p.Wt[0],
-                     w_stride=self.Fin, wT=p.W3[:, 0, :], wT_stride=self.Fo, wT_lo=p.W3_lo[:, 0, :])
+                     w_stride=self.Fin, wT=p.W3[:, 0, :], wT_stride=self.Fo)
         else:
             t = dict(src=g2, op=sk.opsT[0], F=self.Fo, src_rows=sk.rows_out, src_stride=self.Fo, w=None, w_stride=0)
         self.conv1.bwd(x, ycat, dh1, dx=dx, dx_epi=EPI_SLOPE, dx_aux=dx_aux, dycat=dycat, dx_extra=[t])
@@ -929,15 +918,9 @@ class CapeNetwork:
             torch.cuda.current_stream().wait_stream(self.dw_stream)
             self._dw_pending = False
 
-    def lo_of(self, t):
-        r = self.PG.lo_of(t)
-        return r if r is not None else self.PD.lo_of(t)
-
     def prep_weights(self):
-        """Copies derived from the weights (K-major / per-order layouts, tf32 low parts); run after every update:
-        three launches for the whole network."""
-        E.tf32_lo(self.tp, self.PG.flat, self.PG.lo)
-        E.tf32_lo(self.tp, self.PD.flat, self.PD.lo)
+        """Copies derived from the weights (K-major / per-order layouts); run after every update: one launch for the
+        whole network."""
         self.wprep.run()
 
     def scratch_req(self, nfloats):

@@ -34,7 +34,7 @@ def _site(tp, L, K, U, D):
 
 class _ChebFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, W, bias, site, tp, act, precise=False):
+    def forward(ctx, x, W, bias, site, tp, act):
         N, M, Fin = x.shape
         K = site.K
         Fout = W.shape[1]
@@ -42,16 +42,15 @@ class _ChebFn(torch.autograd.Function):
         W = W.contiguous()
         out = torch.empty(N, site.rows_out, Fout, device=x.device)
         W3 = W.view(Fin, K, Fout)
-        Wt, Wt_lo = torch.empty(Fout, K, Fin, device=x.device), torch.empty(Fout, K, Fin, device=x.device)
-        E.weight_transpose(tp, W, Fin, K, Fout, Wt, Wt_lo)
+        Wt = torch.empty(Fout, K, Fin, device=x.device)
+        E.weight_transpose(tp, W, Fin, K, Fout, Wt)
         terms = [dict(src=x, op=site.ops[k], F=Fin, src_rows=site.rows_in, src_stride=Fin, w=W3[:, k, :],
-                      w_stride=K * Fout, wT=Wt[:, k, :], wT_stride=K * Fin, wT_lo=Wt_lo[:, k, :]) for k in range(K)]
+                      w_stride=K * Fout, wT=Wt[:, k, :], wT_stride=K * Fin) for k in range(K)]
         b = bias.contiguous().view(-1) if bias is not None else None
         # one bias per filter ([F] / [1, 1, F]: b1*) or per vertex and filter ([1, M, F]: b2relu, lib/models.py:123-127)
         per_row = b is not None and b.numel() == site.rows_out * Fout and site.rows_out > 1
         assert b is None or per_row or b.numel() == Fout, "bias must be [F], [1, 1, F] or [1, M, F]"
-        E.cheb_call(tp, N, site.rows_out, Fout, terms, out, epilogue=EPI_LINEAR, act=act, bias=b, bias_per_row=per_row,
-                    precise=precise)
+        E.cheb_call(tp, N, site.rows_out, Fout, terms, out, epilogue=EPI_LINEAR, act=act, bias=b, bias_per_row=per_row)
         ctx.save_for_backward(x, W, out)
         ctx.site, ctx.tp, ctx.act, ctx.has_bias, ctx.per_row = site, tp, act, bias is not None, per_row
         ctx.bias_shape = tuple(bias.shape) if bias is not None else None
@@ -86,40 +85,37 @@ class _ChebFn(torch.autograd.Function):
             E.weight_transpose(tp, W, Fin, K, Fout, Wt)
             dx = torch.empty_like(x)
             W3 = W.view(Fin, K, Fout)
-            W_lo = torch.empty_like(W)
-            E.tf32_lo(tp, W, W_lo)
-            W3_lo = W_lo.view(Fin, K, Fout)
             terms = [dict(src=g, op=site.opsT[k], F=Fout, src_rows=site.rows_out, src_stride=Fout, w=Wt[:, k, :],
-                          w_stride=K * Fin, wT=W3[:, k, :], wT_stride=K * Fout, wT_lo=W3_lo[:, k, :]) for k in range(K)]
+                          w_stride=K * Fin, wT=W3[:, k, :], wT_stride=K * Fout) for k in range(K)]
             E.cheb_call(tp, N, site.rows_in, Fin, terms, dx)
-        return dx, dW, db, None, None, None, None
+        return dx, dW, db, None, None, None
 
 
-def chebyshev5(x, L, W, K, bias=None, activation=None, pool=None, unpool=None, precise=False):
+def chebyshev5(x, L, W, K, bias=None, activation=None, pool=None, unpool=None):
     """Chebyshev graph convolution y = sum_k T_k(L~) x W[k::K] (lib/models.py:69-103); W is [Fin*K, Fout] with row
-    index fin*K + k.  precise: short tensor-core accumulation chains (cape_conv_args.precise; K = 1 / plain operands).  Optional fusions: `unpool` U applied to x first (models.py:750,782), `bias`+`activation`
+    index fin*K + k.  Optional fusions: `unpool` U applied to x first (models.py:750,782), `bias`+`activation`
     ('b1leakyrelu' | 'b1relu' | 'b2relu' (bias [1, M, Fout]) | 'b1tanh' | None, models.py:105-127) and `pool` D applied
     last (models.py:168)."""
     tp = topology_for(x.device)
     if activation == "b1tanh":
         # lib/models.py:111-115; unused by every shipped config: the bias rides in the conv's epilogue, the tanh is a
         # separate elementwise pass (and comes before the pooling, as in the reference)
-        y = torch.tanh(chebyshev5(x, L, W, K, bias=bias, activation=None, unpool=unpool, precise=precise))
+        y = torch.tanh(chebyshev5(x, L, W, K, bias=bias, activation=None, unpool=unpool))
         return poolwT(y, pool) if pool is not None else y
     act = {None: ACT_NONE, "b1leakyrelu": ACT_LEAKY, "b1relu": ACT_RELU, "b2relu": ACT_RELU}[activation]
     if pool is not None and bias is not None and bias.numel() > W.shape[1]:
         # a per-vertex bias (b2relu) lives on the un-pooled vertices: conv + bias + activation first, then the pooling
-        y = _ChebFn.apply(x, W, bias, _site(tp, L, K, unpool, None), tp, act, precise)
+        y = _ChebFn.apply(x, W, bias, _site(tp, L, K, unpool, None), tp, act)
         return poolwT(y, pool)
     if pool is not None and (bias is not None or act != ACT_NONE):
         from . import topology as topo
         if not topo.is_selection(pool):
             # pooling commutes with the pointwise bias/activation only for row selections (the reference's D): a
             # general sampling matrix is applied after them, as the reference does (lib/models.py:164-168)
-            y = _ChebFn.apply(x, W, bias, _site(tp, L, K, unpool, None), tp, act, precise)
+            y = _ChebFn.apply(x, W, bias, _site(tp, L, K, unpool, None), tp, act)
             return poolwT(y, pool)
     site = _site(tp, L, K, unpool, pool)
-    return _ChebFn.apply(x, W, bias, site, tp, act, precise)
+    return _ChebFn.apply(x, W, bias, site, tp, act)
 
 
 class _ResampleFn(torch.autograd.Function):

@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define CAPE_ABI_VERSION 3
+#define CAPE_ABI_VERSION 4
 #define CAPE_MAX_TERMS 8
 
 typedef struct cape_topology cape_topology;
@@ -87,10 +87,6 @@ typedef struct {
    * "narrow side" operand (dW_k = x^T (op_k^T G)). */
   float* stash;
   int stash_stride;
-  /* optional: low parts of wT / w2T (x - tf32_trunc(x), same layout; cape_tf32_lo or cape_cheb_weight_transpose
-   * make them).  Accepted for compatibility; the wgmma kernels split the weights on chip and do not read them. */
-  const float* wT_lo;
-  const float* w2T_lo;
 } cape_term;
 
 enum {
@@ -115,11 +111,8 @@ typedef struct {
   const float* aux;    /* [N, rows_out, ncols] (SLOPE / DUALMASK) */
   float* out;          /* [N, rows_out, ncols] */
   float* out2;         /* [N, rows_out, ncols] or NULL */
-  /* Accepted for compatibility and without effect: every tensor-core contraction keeps its accumulation chains short
-   * (a fresh accumulator per 32-deep chunk, summed in fp32 with round-to-nearest), which is what 1 used to ask for. */
-  int precise;
   /* 1: fail (rc < 0) instead of falling back to the gather / fp32-pipe kernels when the plain-operand tensor-core kernel
-   * cannot take the call -- for callers that only filled wT / wT_lo (the `w` pointers are then never read). */
+   * cannot take the call -- for callers that only filled wT / w2T (the `w` pointers are then never read). */
   int plain_only;
 } cape_conv_args;
 
@@ -163,7 +156,7 @@ typedef struct {
 } cape_apply_args;
 int cape_apply(cape_topology* t, const cape_apply_args* a, void* stream);
 
-/* Experiment knobs (process-wide, 16 integer slots, all 0 by default = the shipped configuration).  They switch single
+/* Experiment knobs (process-wide, all 0 by default = the shipped configuration).  They switch single
  * optimisations off for A/B measurements and fallback-path tests: [7]=1 thin-output layers on the generic kernels,
  * [8]=1 no tensor-core plain-operand conv path, [10]=rows per CTA of cape_apply (16..1024), [16]=1 scalar FC kernel,
  * [17]=1 fixed CTA count of the thin weight gradient.  Returns the previous value, <0 for an unknown key. */
@@ -236,9 +229,8 @@ int cape_resample(cape_topology* t, int op, const float* x, int x_stride, float*
                   int rows_in, int F, const float* cond, int C, void* stream);
 
 /* Weight re-layout for the data-gradient pass of chebyshev5: wt[(c*K + k)*Fin + f] = w[(f*K + k)*Fout + c]
- * for f < Fin (rows of w beyond Fin*K -- the condition channels -- are not touched); wt_lo (optional, same layout)
- * receives wt - tf32_trunc(wt). */
-int cape_cheb_weight_transpose(const float* w, int Fin, int K, int Fout, float* wt, float* wt_lo, void* stream);
+ * for f < Fin (rows of w beyond Fin*K -- the condition channels -- are not touched). */
+int cape_cheb_weight_transpose(const float* w, int Fin, int K, int Fout, float* wt, void* stream);
 
 /* The derived weight layouts of MANY layers in one launch (run after every optimiser step).  Per descriptor, from the
  * reference layout w[(f*K + k)*Fout + c] (rows f < Fin; condition rows beyond are not touched):
@@ -246,21 +238,16 @@ int cape_cheb_weight_transpose(const float* w, int Fin, int K, int Fout, float* 
  *                                 [(k, c), f], of the contract-first form Z = X @ [W_0 | W_1 | ...]), fp32-pipe operand of
  *                                 the data-gradient pass;
  *   wk[(k*Fin + f)*Fout + c]   -- per-order plain copies: K-major B operand of the contract-first data gradient
- *                                 Z = G @ [W_0^T | W_1^T | ...];
- * each with its tf32 low part (x - tf32_trunc(x)) for the 3xTF32 scheme.  NULL outputs are skipped.  `descs_device`
+ *                                 Z = G @ [W_0^T | W_1^T | ...].
+ * NULL outputs are skipped.  `descs_device`
  * is a DEVICE array of n descriptors (the pointers never change, so the caller uploads it once). */
 typedef struct {
   const float* w;
   int Fin, K, Fout;
   float* wt;
-  float* wt_lo;
   float* wk;
-  float* wk_lo;
 } cape_wprep;
 int cape_weight_prep(const cape_wprep* descs_device, int n, int blocks_per_desc, void* stream);
-
-/* lo[i] = x[i] - tf32_trunc(x[i]): the second operand of the 3xTF32 scheme for a tensor the tensor cores read raw */
-int cape_tf32_lo(const float* x, float* lo, long long n, void* stream);
 
 /* ---- elementwise helpers ------------------------------------------------------------------------ */
 /* g = dy * (y > 0 ? 1 : alpha)   (backward of leaky_relu given its output) */

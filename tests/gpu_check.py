@@ -36,7 +36,7 @@ def main():
     only = sys.argv[1:]
     jobs = [("golden", lambda: parity.golden_ops(h)), ("gemm", parity.gemm_cases),
             ("cheb", lambda: parity.cheb_grad_cases(h)), ("plain", lambda: parity.plain_operand_cases(h)),
-            ("precise", lambda: parity.precise_vs_truth(h)), ("apply", lambda: parity.apply_cases(h)), ("gn", parity.gn_case), ("tc", lambda: parity.tc_vs_simt(h)),
+            ("plain_fp64", lambda: parity.plain_operand_vs_float64(h)), ("apply", lambda: parity.apply_cases(h)), ("gn", parity.gn_case), ("tc", lambda: parity.tc_vs_simt(h)),
             ("step", lambda: parity.train_step(h, cfg, N=2)),
             ("step_ref", lambda: parity.train_step(h, cfg, N=2, ref_compat=True)),
             ("step_rawinit", lambda: parity.train_step(h, cfg, N=2, fc_scale=1.0)),

@@ -23,9 +23,20 @@ def test_header_symbols_exported(lib_built):
     assert sorted(_lib.SIGNATURES) == names, "ctypes prototypes and header out of sync"
 
 
-def test_abi_version_and_error_string(lib_built):
-    assert lib_built.cape_abi_version() == 3
+def test_abi_v4_and_error_string(lib_built):
+    assert lib_built.cape_abi_version() == 4
     assert isinstance(lib_built.cape_last_error(), bytes)
+
+
+def test_set_tuning_rejects_unknown_keys(lib_built):
+    """cape_set_tuning takes only the documented knobs and returns the previous value of one it takes."""
+    assert lib_built.cape_set_tuning(4, 1) < 0
+    prev = lib_built.cape_set_tuning(7, 0)
+    try:
+        assert prev >= 0
+        assert lib_built.cape_set_tuning(7, 0) == 0
+    finally:
+        lib_built.cape_set_tuning(7, prev)
 
 
 def test_struct_layout_matches_header():

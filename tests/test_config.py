@@ -75,22 +75,6 @@ def test_reference_configs_load_unchanged(tmp_path):
             assert (args.nz, args.nz_cond, args.nz_cond2, args.affine) == (18, 24, 8, 0)
 
 
-def test_param_store_low_part_views():
-    """ParamStore.lo_of: the tf32 low-part buffer is addressed through the same views as the parameters."""
-    import torch
-    from cape_b200.network import ParamStore
-    specs = {"a/weights": (6, 8), "a/bias": (8,), "b/weights": (3, 5)}
-    ps = ParamStore(specs, list(specs), torch.device("cpu"))
-    ps.flat.copy_(torch.arange(ps.size, dtype=torch.float32))
-    ps.lo.copy_(-ps.flat)
-    w = ps.w("b/weights")
-    lo = ps.lo_of(w)
-    assert lo is not None and lo.shape == w.shape and torch.equal(lo, -w)
-    v = ps.w("a/weights").view(6, 8)
-    assert torch.equal(ps.lo_of(v), -v)
-    assert ps.lo_of(torch.zeros(4)) is None                     # not a view of this store
-
-
 def test_weight_gradient_operand_choice():
     """choose_dw_mode on the layer shapes of the shipped config (levels 6890/3445/1723/862)."""
     from cape_b200.network import choose_dw_mode as m

@@ -40,39 +40,12 @@ def test_plain_operand_kernel(hierarchy):
     _assert_all(parity.plain_operand_cases(hierarchy))
 
 
-def test_plain_operand_kernel_without_presplit_weights(hierarchy, monkeypatch):
-    """Same calls with the tf32 low parts of the weights (cape_term.wT_lo) overwritten with NaN: the tensor-core kernels
-    split the weights on chip and must not read them; plus the short-chain accuracy."""
-    import torch
-    from cape_b200 import engine as E
-    transpose, lo = E.weight_transpose, E.tf32_lo
-
-    def transpose_nan(tp, w, Fin, K, Fout, wt, wt_lo=None):
-        transpose(tp, w, Fin, K, Fout, wt, wt_lo)
-        if wt_lo is not None:
-            torch.cuda.synchronize()
-            wt_lo.fill_(float("nan"))
-
-    def lo_nan(tp, x, out):
-        lo(tp, x, out)
-        torch.cuda.synchronize()
-        out.fill_(float("nan"))
-
-    monkeypatch.setattr(E, "weight_transpose", transpose_nan)
-    monkeypatch.setattr(E, "tf32_lo", lo_nan)
-    _assert_all(parity.plain_operand_cases(hierarchy))
-    res = parity.precise_vs_truth(hierarchy)
-    assert res["precise L8 1024->512 (max-rel vs fp64)"] < 4e-6, res
-
-
-def test_precise_accumulation(hierarchy):
-    """cape_conv_args.precise: short tensor-core accumulation chains -- close to fp32 SIMT accuracy on a 1024-long
-    reduction.  The default path accumulates per chunk as well, so it must meet the same bound."""
-    res = parity.precise_vs_truth(hierarchy)
-    assert res["precise L8 1024->512 (max-rel vs fp64)"] < 4e-6, res
-    assert res["default L8 1024->512 (max-rel vs fp64)"] < 4e-6, res
-    assert res["precise L8 512->64 (max-rel vs fp64)"] < 3e-6, res
-    assert res["default L8 512->64 (max-rel vs fp64)"] < 3e-6, res
+def test_plain_operand_accuracy_vs_float64(hierarchy):
+    """Short tensor-core accumulation chains (a fresh accumulator per 32-deep chunk): close to fp32 SIMT accuracy on
+    512- and 1024-long reductions."""
+    res = parity.plain_operand_vs_float64(hierarchy)
+    assert res["L8 1024->512 (max-rel vs fp64)"] < 4e-6, res
+    assert res["L8 512->64 (max-rel vs fp64)"] < 3e-6, res
 
 
 def test_apply_operators(hierarchy):
@@ -129,7 +102,7 @@ def test_train_step_unmasked_forward(hierarchy, cfg, capsys):
 
 
 def test_three_consecutive_updates(hierarchy, cfg):
-    """Momentum != 0, warm-up learning rates, refreshed K-major / tf32-low weight copies: three updates in a row with
+    """Momentum != 0, warm-up learning rates, refreshed K-major weight copies: three updates in a row with
     fresh batches, every update compared with the oracle carrying its own state (lib/models.py:460-472)."""
     _assert_all(parity.train_step(hierarchy, cfg, N=2, nsteps=3, fc_scale=1.0))
 

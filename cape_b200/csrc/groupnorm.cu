@@ -1,8 +1,11 @@
 // Group normalisation + ReLU for the non-affine decoder residual blocks
 // (CAPE.gn at lib/models.py:681-712 followed by tf.nn.relu at :752,756,760).
 // Layout [N, rows, C]: the statistics of group g of sample n span (C/G contiguous channels) x (all rows),
-// biased variance (tf.nn.moments), eps inside the sqrt.  Group sums are accumulated in fp64 so the
-// E[x^2]-E[x]^2 form stays within fp32 rounding of the two-pass reference.
+// biased variance (tf.nn.moments), eps inside the sqrt.  The statistics pass sums, per channel, the deviations from a
+// pivot (the channel's value in the first row of the block) in fp32 registers and turns them into raw moments in fp64
+// before the group sums, which are fp64 too.  So the fp32 sums only see the spread within a channel, never its offset:
+// mean and variance stay within fp32 rounding of the two-pass reference however large |mean| / std is (data far from
+// zero, and the condition channels of GNBlock, which are constant over the vertices).
 #include "common.cuh"
 
 namespace cape {
@@ -10,21 +13,25 @@ namespace cape {
 constexpr int GN_ROWS = 64;      // rows per CTA in the reduction passes
 constexpr int GN_MAXG = 32;
 
-// Partial sums of one block of rows: thread = (row slot, float4 column); per-thread register sums over its rows, a
-// shared-memory reduction over the row slots, then one fp64 atomic per group and block.
+// Partial sums of one block of rows: thread = (row slot, float4 column); per-thread register sums of d = x - p over its
+// rows (p = the block's first row, per channel), a shared-memory reduction over the row slots, then per channel
+// sum(x) = S + m p and sum(x^2) = Q + 2 p S + m p^2 in fp64 (m rows) and one fp64 atomic per group and block.
 __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ x, int rows, int C, int G,
                                                        int rows_per_block, double* __restrict__ acc) {
   __shared__ float red[2][1024];
   const int n = blockIdx.y, cpr = C >> 2, rslots = min(256 / cpr, 32);
   const int rs = threadIdx.x / cpr, c4 = threadIdx.x % cpr;
   const int r0 = blockIdx.x * rows_per_block, r1 = min(rows, r0 + rows_per_block);
+  const float* xb = x + ((size_t)n * rows + r0) * C;             // row r0 of sample n: the pivots
   float s[4] = {0.f, 0.f, 0.f, 0.f}, q[4] = {0.f, 0.f, 0.f, 0.f};
   if (rs < rslots) {
-    const float4* xp = reinterpret_cast<const float4*>(x + (size_t)n * rows * C) + c4;
-    for (int r = r0 + rs; r < r1; r += rslots) {
+    const float4* xp = reinterpret_cast<const float4*>(xb) + c4;
+    const float4 p = __ldg(xp);
+    for (int r = rs; r < r1 - r0; r += rslots) {
       const float4 v = __ldg(xp + (size_t)r * cpr);
-      s[0] += v.x; s[1] += v.y; s[2] += v.z; s[3] += v.w;
-      q[0] = fmaf(v.x, v.x, q[0]); q[1] = fmaf(v.y, v.y, q[1]); q[2] = fmaf(v.z, v.z, q[2]); q[3] = fmaf(v.w, v.w, q[3]);
+      const float d[4] = {v.x - p.x, v.y - p.y, v.z - p.z, v.w - p.w};
+#pragma unroll
+      for (int j = 0; j < 4; ++j) { s[j] += d[j]; q[j] = fmaf(d[j], d[j], q[j]); }
     }
 #pragma unroll
     for (int j = 0; j < 4; ++j) { red[0][rs * C + c4 * 4 + j] = s[j]; red[1][rs * C + c4 * 4 + j] = q[j]; }
@@ -32,9 +39,15 @@ __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__
   __syncthreads();
   if (threadIdx.x < G) {
     const int cpg = C / G;
+    const double m = (double)(r1 - r0);
     double ds = 0.0, dq = 0.0;
-    for (int c = threadIdx.x * cpg; c < (threadIdx.x + 1) * cpg; ++c)
-      for (int k = 0; k < rslots; ++k) { ds += (double)red[0][k * C + c]; dq += (double)red[1][k * C + c]; }
+    for (int c = threadIdx.x * cpg; c < (threadIdx.x + 1) * cpg; ++c) {
+      double S = 0.0, Q = 0.0;
+      for (int k = 0; k < rslots; ++k) { S += (double)red[0][k * C + c]; Q += (double)red[1][k * C + c]; }
+      const double p = (double)__ldg(xb + c);
+      ds += S + m * p;
+      dq += Q + p * (2.0 * S + m * p);
+    }
     atomicAdd(acc + ((size_t)n * G + threadIdx.x) * 2 + 0, ds);
     atomicAdd(acc + ((size_t)n * G + threadIdx.x) * 2 + 1, dq);
   }

@@ -10,10 +10,12 @@ shapes and compared with a float64 NumPy / SciPy product:
   grid-stride loop, condition slots, bias, activation;
 - cape_colsum, cape_resample with a condition, cape_gemm_batch.
 
-Every case checks which kernels ran (CUDA activity tracing and cape_launch_count), that every element it should write
+Every case checks which kernels ran (CUDA activity tracing, or the nodes of a CUDA graph captured from the same call
+when the trace has lost records, and cape_launch_count), that every element it should write
 is finite and within 1e-4 of max |truth|, and that sentinels around and after its outputs are untouched.  Calls the
 thin kernels reject are checked to take the generic kernels and still give the float64 result."""
 import contextlib
+import ctypes
 
 import numpy as np
 import pytest
@@ -79,8 +81,9 @@ def _traced(fn, reset, attempts=3):
     """Runs fn() under CUDA activity tracing; returns the short names of the library's kernels it launched, in order,
     checked against the library's own launch counter.  A trace now and then lacks the record of the first kernel
     launched after tracing starts, so a torch kernel goes first; if records are still missing, reset() restores the
-    outputs and the call runs again, and after `attempts` incomplete traces the case fails (the kernel selection could
-    not be checked)."""
+    outputs and the call runs again.  The profiler also returns whole sessions without device records at times; after
+    `attempts` incomplete traces fn() runs once more for its outputs and the names are read from a CUDA graph captured
+    from a further call (_captured), which does not depend on activity records."""
     from torch.profiler import ProfilerActivity, profile
     lib = _lib()
     for _ in range(attempts):
@@ -99,8 +102,86 @@ def _traced(fn, reset, attempts=3):
         print("incomplete trace (%d launches counted, kernels %s): again" % (launched, names))
         reset()
         torch.cuda.synchronize()
-    pytest.fail("the CUDA profiler recorded %d of the %d kernels launched in each of %d traces: cannot tell which "
-                "kernels ran" % (len(names), launched, attempts))
+    torch.cuda.synchronize()
+    n0 = lib.cape_launch_count()
+    fn()
+    torch.cuda.synchronize()
+    launched = lib.cape_launch_count() - n0
+    names = _captured(fn)
+    assert len(names) == launched, "captured kernels %s, %d launches counted" % (names, launched)
+    return names
+
+
+class _KernelNodeParams(ctypes.Structure):
+    """CUDA_KERNEL_NODE_PARAMS_v2 (cuda.h)."""
+    _fields_ = [("func", ctypes.c_void_p), ("gridDimX", ctypes.c_uint), ("gridDimY", ctypes.c_uint),
+                ("gridDimZ", ctypes.c_uint), ("blockDimX", ctypes.c_uint), ("blockDimY", ctypes.c_uint),
+                ("blockDimZ", ctypes.c_uint), ("sharedMemBytes", ctypes.c_uint), ("kernelParams", ctypes.c_void_p),
+                ("extra", ctypes.c_void_p), ("kern", ctypes.c_void_p), ("ctx", ctypes.c_void_p)]
+
+
+def _captured(fn):
+    """Short names of the library's kernels fn() launches, in launch order, read from the kernel nodes of a CUDA graph
+    captured (relaxed mode, on a side stream) from one call of fn().  The graph is never launched: this call of fn()
+    has no effect on the device (host-side set-up such as a first upload must have happened in an earlier call).  Driver API through ctypes; names demangled with the C++ runtime's __cxa_demangle."""
+    cu = ctypes.CDLL("libcuda.so.1")
+    cxx = ctypes.CDLL("libstdc++.so.6")
+    cxx.__cxa_demangle.restype = ctypes.c_void_p
+    cxx.__cxa_demangle.argtypes = [ctypes.c_char_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_int)]
+    libc = ctypes.CDLL(None)
+    libc.free.argtypes = [ctypes.c_void_p]
+    vp = ctypes.c_void_p
+    pp, sz = ctypes.POINTER(ctypes.c_void_p), ctypes.POINTER(ctypes.c_size_t)
+    for fname, args in (("cuStreamBeginCapture_v2", [vp, ctypes.c_int]), ("cuStreamEndCapture", [vp, pp]),
+                        ("cuGraphGetNodes", [vp, pp, sz]), ("cuGraphNodeGetType", [vp, ctypes.POINTER(ctypes.c_int)]),
+                        ("cuGraphKernelNodeGetParams_v2", [vp, ctypes.POINTER(_KernelNodeParams)]),
+                        ("cuFuncGetName", [ctypes.POINTER(ctypes.c_char_p), vp]),
+                        ("cuKernelGetName", [ctypes.POINTER(ctypes.c_char_p), vp]), ("cuGraphDestroy", [vp])):
+        getattr(cu, fname).argtypes = args
+        getattr(cu, fname).restype = ctypes.c_int
+
+    def ok(rc, what):
+        assert rc == 0, "%s: CUresult %d" % (what, rc)
+
+    torch.cuda.synchronize()
+    s = torch.cuda.Stream(device=_dev())
+    graph = vp()
+    with torch.cuda.stream(s):
+        h = vp(s.cuda_stream)
+        ok(cu.cuStreamBeginCapture_v2(h, 2), "cuStreamBeginCapture")          # CU_STREAM_CAPTURE_MODE_RELAXED
+        try:
+            fn()
+        finally:
+            ok(cu.cuStreamEndCapture(h, ctypes.byref(graph)), "cuStreamEndCapture")
+    try:
+        n = ctypes.c_size_t(0)
+        ok(cu.cuGraphGetNodes(graph, None, ctypes.byref(n)), "cuGraphGetNodes")
+        nodes = (vp * max(n.value, 1))()
+        ok(cu.cuGraphGetNodes(graph, ctypes.cast(nodes, pp), ctypes.byref(n)), "cuGraphGetNodes")
+        order = [nodes[i] for i in range(n.value)]       # creation order: the order of the launches
+        names = []
+        for nd in order:
+            t = ctypes.c_int(-1)
+            ok(cu.cuGraphNodeGetType(vp(nd), ctypes.byref(t)), "cuGraphNodeGetType")
+            if t.value != 0:                                # CU_GRAPH_NODE_TYPE_KERNEL
+                continue
+            p = _KernelNodeParams()
+            ok(cu.cuGraphKernelNodeGetParams_v2(vp(nd), ctypes.byref(p)), "cuGraphKernelNodeGetParams")
+            raw = ctypes.c_char_p()
+            if p.func:
+                ok(cu.cuFuncGetName(ctypes.byref(raw), vp(p.func)), "cuFuncGetName")
+            else:
+                ok(cu.cuKernelGetName(ctypes.byref(raw), vp(p.kern)), "cuKernelGetName")
+            status = ctypes.c_int(-1)
+            dm = cxx.__cxa_demangle(raw.value, None, None, ctypes.byref(status))
+            name = ctypes.string_at(dm).decode() if status.value == 0 else raw.value.decode()
+            if dm:
+                libc.free(dm)
+            if "cape::" in name:
+                names.append(_short(name))
+        return names
+    finally:
+        cu.cuGraphDestroy(graph)
 
 
 def _ran(names, kernel):

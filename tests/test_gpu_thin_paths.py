@@ -185,7 +185,10 @@ def _captured(fn):
 
 
 def _ran(names, kernel):
-    return any(n == kernel or n.startswith(kernel + "<") for n in names)
+    """kernel: a name (any of its template instances) or one instance, e.g. 'ellconv_kernel<32, true, false>' (spaces in
+    the template arguments are ignored)."""
+    k = kernel.replace(" ", "")
+    return any(n.replace(" ", "") == k or ("<" not in k and n.startswith(k + "<")) for n in names)
 
 
 def _expect(names, kernels=(), launches=None, thin=None):

@@ -141,20 +141,20 @@ def test_res_affine_model_update_at_batch_64_matches_oracle(hierarchy):
     _assert_parity(res, "res_affine N=64")
 
 
-@pytest.mark.parametrize("tag", ["default", "res_affine"])
-def test_update_matches_the_reference_golden(hierarchy, tag):
-    """The update ref_models_golden_3.npz holds, on the CUDA path: x_hat, the losses and the discriminator's post-update
-    parameters (what parity.reference_golden_update compares for the shipped models, for the same reasons)."""
+def golden_update_errors(h, configs, load, tag):
+    """Relative errors of the CUDA update against a reference golden file written by make_ref_golden_resblock.py or
+    a generator built like it (`configs()` / `load()` of that module): x_hat, the losses and the discriminator's
+    post-update parameters (what parity.reference_golden_update compares for the shipped models, for the same
+    reasons)."""
     from cape_b200.network import CapeNetwork
-    cfg, N, step = next((c, n, s) for t, c, n, s in G3.configs() if t == tag)
-    h = hierarchy
+    cfg, N, step = next((c, n, s) for t, c, n, s in configs() if t == tag)
     params, batch = G.inputs(cfg, h, N)
     net = CapeNetwork(h["L"], h["D"], h["U"], h["L_d"], h["D_d"], cfg, N, params=params, ref_compat=True)
     tb = {k: torch.from_numpy(v) for k, v in batch.items()}
     net.set_inputs(tb["x_g"], tb["cond_g"], tb["cond2_g"], tb["eps"], tb["x_d"], tb["cond_d"], tb["cond2_d"])
     net.train_step(step=step)
     torch.cuda.synchronize()
-    z = G3.load()
+    z = load()
     out = {"x_hat (vertex-L2)": parity.vertex_l2(net.x_hat.cpu().numpy(), z[tag + "/x_hat"])}
     got = net.loss_dict()
     for k in ("recon", "edge", "latent", "gan_g", "gan_d"):
@@ -168,6 +168,13 @@ def test_update_matches_the_reference_golden(hierarchy, tag):
             out["param " + name] = parity.rel(v if base + "#full" in z else v[G.sample_index(name, v.size)],
                                               ref.reshape(-1))
     print("%s vs reference: worst %s" % (tag, max(out.items(), key=lambda kv: kv[1])))
+    return out
+
+
+@pytest.mark.parametrize("tag", ["default", "res_affine"])
+def test_update_matches_the_reference_golden(hierarchy, tag):
+    """The update ref_models_golden_3.npz holds, on the CUDA path."""
+    out = golden_update_errors(hierarchy, G3.configs, G3.load, tag)
     assert max(out.values()) < parity.TOL, {k: v for k, v in out.items() if not v < parity.TOL}
 
 

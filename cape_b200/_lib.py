@@ -8,8 +8,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("CAPE_B200_LIB") or os.path.join(_HERE, "libcape_b200.so")
 
 MAX_TERMS = 8
-EPI_LINEAR, EPI_AFFINE, EPI_SLOPE, EPI_DUALMASK = 0, 1, 2, 3
-ACT_NONE, ACT_LEAKY, ACT_RELU = 0, 1, 2
+EPI_LINEAR, EPI_AFFINE, EPI_SLOPE, EPI_DUALMASK, EPI_TANHGRAD = 0, 1, 2, 3, 4
+ACT_NONE, ACT_LEAKY, ACT_RELU, ACT_TANH = 0, 1, 2, 3
+RECON_L1, RECON_L2, RECON_HUBER = 0, 1, 2
 
 f32p = C.c_void_p  # device pointers travel as integers
 
@@ -95,6 +96,9 @@ SIGNATURES = {
     "cape_recon_losses": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float,
                                     C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_void_p]),
+    "cape_recon_losses_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                       C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
     "cape_bce_logits": (C.c_int, [C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cape_sumsq": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "cape_sgd_clip_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float,

@@ -62,7 +62,7 @@ __device__ __forceinline__ void ap_advance(int& r, int& n, int by, int rows) {
   while (r >= rows) { r -= rows; ++n; }
 }
 
-template <bool DUAL>
+template <bool DUAL, bool TANH>
 __device__ __forceinline__ void ap_store(const ApParams& p, long long R, int r, int c, float4 a0, float4 a1) {
   const size_t o = (size_t)R * p.out_stride + c;
   float v0[4] = {a0.x, a0.y, a0.z, a0.w}, v1[4] = {a1.x, a1.y, a1.z, a1.w}, o1[4], o2[4];
@@ -74,6 +74,7 @@ __device__ __forceinline__ void ap_store(const ApParams& p, long long R, int r, 
       if (p.bias != nullptr) v += __ldg(p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) + c + j);
       if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
       else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
+      else if (TANH && p.act == CAPE_ACT_TANH) v = tanhf(v);
       o1[j] = v;
     }
   } else if (p.epilogue == CAPE_EPI_AFFINE) {
@@ -90,6 +91,9 @@ __device__ __forceinline__ void ap_store(const ApParams& p, long long R, int r, 
     if (p.epilogue == CAPE_EPI_SLOPE) {
 #pragma unroll
       for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (a[j] > 0.f ? 1.f : p.alpha);
+    } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
+#pragma unroll
+      for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (1.f - a[j] * a[j]);
     } else {
       write2 = p.out2 != nullptr;
 #pragma unroll
@@ -100,7 +104,8 @@ __device__ __forceinline__ void ap_store(const ApParams& p, long long R, int r, 
   if (write2) *reinterpret_cast<float4*>(p.out2 + o) = make_float4(o2[0], o2[1], o2[2], o2[3]);
 }
 
-template <bool DUAL>
+// TANH: the tanh epilogues (b1tanh), compiled only into instantiations of their own (as in conv_wg_kernel)
+template <bool DUAL, bool TANH>
 __global__ void __launch_bounds__(AP_THREADS, 3) apply_kernel(const __grid_constant__ ApParams p) {
   __shared__ __align__(16) float qs[AP_QS];
   const int AP_R = p.rows_cta;
@@ -166,8 +171,8 @@ __global__ void __launch_bounds__(AP_THREADS, 3) apply_kernel(const __grid_const
       else { f4_axpy(a0, tm.scale, ta); f4_axpy(b0, tm.scale, tb); }
     }
     if (p.term_stride > 0) continue;
-    ap_store<DUAL>(p, Ra, ra, c, a0, a1);
-    if (vb) ap_store<DUAL>(p, Rb, rb, c, b0, b1);
+    ap_store<DUAL, TANH>(p, Ra, ra, c, a0, a1);
+    if (vb) ap_store<DUAL, TANH>(p, Rb, rb, c, b0, b1);
   }
 }
 
@@ -183,7 +188,8 @@ extern "C" int cape_apply(cape_topology* t, const cape_apply_args* a, void* stre
   CAPE_REQUIRE(a->nterms >= 1 && a->nterms <= CAPE_MAX_TERMS, "nterms out of range");
   CAPE_REQUIRE(a->out != nullptr, "out is null");
   CAPE_REQUIRE(a->ncols % 4 == 0 && a->ncols <= 4 * AP_THREADS, "cape_apply needs ncols % 4 == 0 and ncols <= 1024");
-  CAPE_REQUIRE(a->epilogue >= CAPE_EPI_LINEAR && a->epilogue <= CAPE_EPI_DUALMASK, "unknown epilogue");
+  CAPE_REQUIRE(a->epilogue >= CAPE_EPI_LINEAR && a->epilogue <= CAPE_EPI_TANHGRAD, "unknown epilogue");
+  CAPE_REQUIRE(a->act >= CAPE_ACT_NONE && a->act <= CAPE_ACT_TANH, "unknown activation");
   ApParams p{};
   p.N = a->N; p.rows_out = a->rows_out; p.ncols = a->ncols; p.nterms = a->nterms;
   p.total_rows = (long long)a->N * a->rows_out;
@@ -226,14 +232,21 @@ extern "C" int cape_apply(cape_topology* t, const cape_apply_args* a, void* stre
                  a->act == CAPE_ACT_NONE && p.nslots == 0 && !dual,
                  "separate outputs (term_stride) take plain terms: LINEAR epilogue, no bias / activation / condition");
   }
-  if (a->epilogue == CAPE_EPI_SLOPE || a->epilogue == CAPE_EPI_DUALMASK) {
+  if (a->epilogue == CAPE_EPI_SLOPE || a->epilogue == CAPE_EPI_DUALMASK || a->epilogue == CAPE_EPI_TANHGRAD) {
     CAPE_REQUIRE(a->aux && aligned16(a->aux), "epilogue needs a 16-byte aligned aux");
-    CAPE_REQUIRE(p.out_stride == a->ncols, "SLOPE / DUALMASK epilogues need out_stride == ncols");
+    CAPE_REQUIRE(p.out_stride == a->ncols, "SLOPE / DUALMASK / TANHGRAD epilogues need out_stride == ncols");
   }
   const long long blocks = (p.total_rows + p.rows_cta - 1) / p.rows_cta;
   CAPE_REQUIRE(blocks < (1LL << 31), "grid too large");
-  if (dual) apply_kernel<true><<<(unsigned)blocks, AP_THREADS, 0, (cudaStream_t)stream>>>(p);
-  else apply_kernel<false><<<(unsigned)blocks, AP_THREADS, 0, (cudaStream_t)stream>>>(p);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool tanh = a->act == CAPE_ACT_TANH || a->epilogue == CAPE_EPI_TANHGRAD;
+  if (dual) {
+    if (tanh) apply_kernel<true, true><<<(unsigned)blocks, AP_THREADS, 0, st>>>(p);
+    else apply_kernel<true, false><<<(unsigned)blocks, AP_THREADS, 0, st>>>(p);
+  } else {
+    if (tanh) apply_kernel<false, true><<<(unsigned)blocks, AP_THREADS, 0, st>>>(p);
+    else apply_kernel<false, false><<<(unsigned)blocks, AP_THREADS, 0, st>>>(p);
+  }
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   return 0;

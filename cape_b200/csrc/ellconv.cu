@@ -282,6 +282,7 @@ __global__ void __launch_bounds__(NT, DUAL ? 1 : 2) ellconv_kernel(const __grid_
           v += __ldg(p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) + c0 + j);
         if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
         else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
+        else if (!DUAL && p.act == CAPE_ACT_TANH) v = tanhf(v);   // DUAL: refused by cape_cheb_fwd
         o1[j] = v;
       }
     } else if (p.epilogue == CAPE_EPI_AFFINE) {
@@ -304,6 +305,9 @@ __global__ void __launch_bounds__(NT, DUAL ? 1 : 2) ellconv_kernel(const __grid_
       if (p.epilogue == CAPE_EPI_SLOPE) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (ax[j] > 0.f ? 1.f : p.alpha);
+      } else if (!DUAL && p.epilogue == CAPE_EPI_TANHGRAD) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (1.f - ax[j] * ax[j]);
       } else {  // DUALMASK
         write2 = p.out2 != nullptr;
 #pragma unroll
@@ -738,9 +742,11 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
   p.epilogue = a->epilogue; p.act = a->act; p.alpha = a->alpha;
   p.bias = a->bias; p.bias_per_row = a->bias_per_row;
   p.aux = a->aux; p.out = a->out; p.out2 = a->out2;
-  CAPE_REQUIRE(a->epilogue >= CAPE_EPI_LINEAR && a->epilogue <= CAPE_EPI_DUALMASK, "unknown epilogue");
+  CAPE_REQUIRE(a->epilogue >= CAPE_EPI_LINEAR && a->epilogue <= CAPE_EPI_TANHGRAD, "unknown epilogue");
+  CAPE_REQUIRE(a->act >= CAPE_ACT_NONE && a->act <= CAPE_ACT_TANH, "unknown activation");
   if (a->epilogue == CAPE_EPI_AFFINE) CAPE_REQUIRE(dual, "AFFINE epilogue needs a w2 term");
-  if (a->epilogue == CAPE_EPI_SLOPE || a->epilogue == CAPE_EPI_DUALMASK) CAPE_REQUIRE(a->aux, "epilogue needs aux");
+  if (a->epilogue == CAPE_EPI_SLOPE || a->epilogue == CAPE_EPI_DUALMASK || a->epilogue == CAPE_EPI_TANHGRAD)
+    CAPE_REQUIRE(a->aux, "epilogue needs aux");
   p.wvec = wvec ? 1 : 0;
   p.ovec = (a->ncols % 4 == 0) && aligned16(a->out) && (!a->out2 || aligned16(a->out2)) && (!a->aux || aligned16(a->aux));
   const int BNsel = a->ncols <= 32 ? 32 : 64;
@@ -765,6 +771,10 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
     rc = launch_ellconv_tc(t, p, dual, st);               // wgmma path when eligible (writes the stashes itself)
     if (rc != 0) return rc < 0 ? rc : 0;
   }
+  // the fp32-pipe kernel with two accumulators (the affine block's forward) has no tanh epilogues: they would cost it
+  // registers it spills already
+  CAPE_REQUIRE(!dual || (a->act != CAPE_ACT_TANH && a->epilogue != CAPE_EPI_TANHGRAD),
+               "tanh / TANHGRAD epilogues with a w2 term need the tensor-core kernel (ncols % 32 == 0, wT / w2T given)");
   if (any_stash) {                                        // fp32-pipe path: the basis copies come from the resample kernel
     for (int i = 0; i < p.nterms; ++i) {
       const TermDev& d = p.terms[i];

@@ -127,7 +127,7 @@ __device__ __forceinline__ void ell_gather4_pairs(const OpView& op, const int (&
 // Tiles come from *counter, which is 0 at the start of a launch: each CTA draws tickets until one is past the last
 // tile, so a launch draws exactly ntiles + gridDim.x tickets, and the CTA that draws the last one resets the counter
 // for the next launch of the handle.
-template <int BN, bool DUAL, bool PASS>
+template <int BN, bool DUAL, bool PASS, bool TANH>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_constant__ ConvParams p,
                                                                   const __grid_constant__ WeightMaps maps, int nqs,
                                                                   int ncol_tiles, int ntiles, unsigned* counter) {
@@ -277,7 +277,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   setmaxnreg_inc<CONSUMER_REGS>();
   const int cw = wg - 2, ctid = tid - PRODUCER_THREADS;
   const bool linear = p.epilogue == CAPE_EPI_LINEAR;
-  const bool use_aux = p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK;
+  const bool use_aux =
+      p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK || (TANH && p.epilogue == CAPE_EPI_TANHGRAD);
   uint32_t it = 0;                            // as the producers' count
   for (;;) {
     mbar_wait(&full[it % S], (it / S) & 1);   // the tile's first chunk carries its index
@@ -411,6 +412,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
             float v = v0[e] + (bias_row != nullptr ? __ldg(bias_row + c + e) : 0.f);
             if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
             else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
+            else if (TANH && p.act == CAPE_ACT_TANH) v = tanhf(v);
             o1[e] = v;
           }
         } else if (p.epilogue == CAPE_EPI_AFFINE) {
@@ -427,6 +429,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
           if (p.epilogue == CAPE_EPI_SLOPE) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) o1[e] = v0[e] * (a2[e] > 0.f ? 1.f : p.alpha);
+          } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) o1[e] = v0[e] * (1.f - a2[e] * a2[e]);
           } else {
             write2 = p.out2 != nullptr;
 #pragma unroll
@@ -476,8 +481,8 @@ int encode_weight_map(CUtensorMap* m, const float* wT, int F, int stride, int nc
   return 0;
 }
 
-template <int BN, bool DUAL, bool PASS = false>
-int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
+template <int BN, bool DUAL, bool PASS, bool TANH>
+int launch_conv_inst(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
   using Cfg = ConvCfg<BN, DUAL>;
   WeightMaps maps;
   memset(&maps, 0, sizeof(maps));
@@ -497,7 +502,7 @@ int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
   const int smem = 1024 + Cfg::RING + BAR_BYTES + nqs * 4;
   static bool configured = false;
   if (!configured) {
-    CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL, PASS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL, PASS, TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          1024 + Cfg::RING + BAR_BYTES + QS_MAX_FLOATS * 4));
     configured = true;
   }
@@ -509,11 +514,19 @@ int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
     return -1;
   }
   const int grid = (int)std::min<long long>(ntiles, t->sm_count);
-  conv_wg_kernel<BN, DUAL, PASS><<<grid, CONV_THREADS, smem, st>>>(p, maps, nqs, ncol_tiles, (int)ntiles,
+  conv_wg_kernel<BN, DUAL, PASS, TANH><<<grid, CONV_THREADS, smem, st>>>(p, maps, nqs, ncol_tiles, (int)ntiles,
                                                                    t->tile_counter);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;
+}
+
+// the tanh epilogues (b1tanh) in instantiations of their own: the precise tanhf, unrolled over a tile's columns, adds a
+// fifth to the kernel's code, which made the other activations' steps ~1 % slower as a run-time branch
+template <int BN, bool DUAL, bool PASS = false>
+int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
+  if (p.act == CAPE_ACT_TANH || p.epilogue == CAPE_EPI_TANHGRAD) return launch_conv_inst<BN, DUAL, PASS, true>(t, p, st);
+  return launch_conv_inst<BN, DUAL, PASS, false>(t, p, st);
 }
 
 // column tile width: the whole output row up to 128 columns (64 with two accumulators), so that the running sums and

@@ -318,6 +318,9 @@ extern "C" int cape_gemm(cape_topology* t, int M, int N, int K, const float* a, 
   CAPE_REQUIRE(M > 0 && N > 0 && K > 0, "empty problem");
   CAPE_REQUIRE(a_cs == 1 || a_rs == 1, "A needs a unit stride");
   CAPE_REQUIRE(b_cs == 1 || b_rs == 1, "B needs a unit stride");
+  // the dense layers of the reference are fixed to leaky ReLU or none (models.py:496-510,557-582): no tanh here
+  CAPE_REQUIRE(act == CAPE_ACT_NONE || act == CAPE_ACT_LEAKY || act == CAPE_ACT_RELU,
+               "cape_gemm implements ACT_NONE, ACT_LEAKY and ACT_RELU");
   GemmParams p{};
   p.M = M; p.N = N; p.K = K;
   p.a = a; p.a_rs = a_rs; p.a_cs = a_cs;

@@ -64,7 +64,8 @@ struct ReconParams {
   const float* pred;
   const float* gt;
   int N, rows;
-  float g_l1;     // lambda_l1 / (N*rows*3)
+  float g_l1;     // lambda_recon / (N*rows*3)
+  float delta;    // Huber threshold
   float g_edge;   // lambda_edge / (N*n_edges)
   float s_l1;     // 1 / (N*rows*3)
   float s_edge;   // 0.5 / (N*n_edges)   (every undirected edge is visited from both ends)
@@ -72,6 +73,24 @@ struct ReconParams {
   float* losses;
 };
 
+// the reconstruction term's value and gradient (before the lambda / count scale) of one coordinate's residual d
+template <int KIND>
+__device__ __forceinline__ float recon_term(float d, float delta, float* grad) {
+  if (KIND == CAPE_RECON_L2) {
+    *grad = 2.f * d;
+    return d * d;
+  }
+  const float a = fabsf(d);
+  if (KIND == CAPE_RECON_HUBER) {
+    const float q = fminf(a, delta);
+    *grad = fminf(fmaxf(d, -delta), delta);
+    return 0.5f * q * q + delta * (a - q);
+  }
+  *grad = (float)((d > 0.f) - (d < 0.f));
+  return a;
+}
+
+template <int KIND>
 __global__ void __launch_bounds__(256) recon_kernel(const __grid_constant__ ReconParams p) {
   __shared__ float red[8];
   const long long total = (long long)p.N * p.rows;
@@ -82,10 +101,13 @@ __global__ void __launch_bounds__(256) recon_kernel(const __grid_constant__ Reco
     const float* pp = p.pred + (size_t)n * p.rows * 3;
     const float* gg = p.gt + (size_t)n * p.rows * 3;
     const float dx = pp[v * 3] - gg[v * 3], dy = pp[v * 3 + 1] - gg[v * 3 + 1], dz = pp[v * 3 + 2] - gg[v * 3 + 2];
-    l1 = fabsf(dx) + fabsf(dy) + fabsf(dz);
-    float gx = p.g_l1 * ((dx > 0.f) - (dx < 0.f));
-    float gy = p.g_l1 * ((dy > 0.f) - (dy < 0.f));
-    float gz = p.g_l1 * ((dz > 0.f) - (dz < 0.f));
+    float tx, ty, tz;
+    const float vx = recon_term<KIND>(dx, p.delta, &tx), vy = recon_term<KIND>(dy, p.delta, &ty),
+                vz = recon_term<KIND>(dz, p.delta, &tz);
+    l1 = vx + vy + vz;
+    float gx = p.g_l1 * tx;
+    float gy = p.g_l1 * ty;
+    float gz = p.g_l1 * tz;
     const int32_t* nb = p.nbr + (size_t)v * p.width;
     for (int j = 0; j < p.width; ++j) {
       const int u = __ldg(nb + j);
@@ -325,10 +347,13 @@ extern "C" int cape_vae_sample_bwd(const float* dz, int dz_stride, const float* 
   return 0;
 }
 
-extern "C" int cape_recon_losses(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
-                                 float lambda_l1, float lambda_edge, int n_edges, const float* mean,
-                                 const float* logvar, int nz, float* dpred, float* losses, void* stream) {
+extern "C" int cape_recon_losses_ex(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
+                                    int kind, float delta, float lambda_l1, float lambda_edge, int n_edges,
+                                    const float* mean, const float* logvar, int nz, float* dpred, float* losses,
+                                    void* stream) {
   CAPE_REQUIRE(t && pred && gt && dpred && losses, "null pointer");
+  CAPE_REQUIRE(kind == CAPE_RECON_L1 || kind == CAPE_RECON_L2 || kind == CAPE_RECON_HUBER, "unknown reconstruction loss");
+  CAPE_REQUIRE(kind != CAPE_RECON_HUBER || delta > 0.f, "the Huber loss needs delta > 0");
   CAPE_REQUIRE(nbr_op >= 0 && nbr_op < (int)t->ops.size(), "bad neighbour operator");
   const EllOp& o = t->ops[nbr_op];
   CAPE_REQUIRE(o.rows_out == rows && o.rows_in == rows, "neighbour operator shape mismatch");
@@ -338,10 +363,14 @@ extern "C" int cape_recon_losses(cape_topology* t, int nbr_op, const float* pred
   const double cnt = (double)N * rows * 3.0, ecnt = (double)N * n_edges;
   p.g_l1 = (float)(lambda_l1 / cnt); p.g_edge = (float)(lambda_edge / ecnt);
   p.s_l1 = (float)(1.0 / cnt); p.s_edge = (float)(0.5 / ecnt);
+  p.delta = delta;
   p.dpred = dpred; p.losses = losses;
   const long long total = (long long)N * rows;
   cudaStream_t st = (cudaStream_t)stream;
-  recon_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(p);
+  const unsigned blocks = (unsigned)((total + 255) / 256);
+  if (kind == CAPE_RECON_L2) recon_kernel<CAPE_RECON_L2><<<blocks, 256, 0, st>>>(p);
+  else if (kind == CAPE_RECON_HUBER) recon_kernel<CAPE_RECON_HUBER><<<blocks, 256, 0, st>>>(p);
+  else recon_kernel<CAPE_RECON_L1><<<blocks, 256, 0, st>>>(p);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   if (mean && logvar && nz > 0) {
@@ -350,6 +379,13 @@ extern "C" int cape_recon_losses(cape_topology* t, int nbr_op, const float* pred
   cape::count_launches(1);
   }
   return 0;
+}
+
+extern "C" int cape_recon_losses(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
+                                 float lambda_l1, float lambda_edge, int n_edges, const float* mean,
+                                 const float* logvar, int nz, float* dpred, float* losses, void* stream) {
+  return cape_recon_losses_ex(t, nbr_op, pred, gt, N, rows, CAPE_RECON_L1, 0.f, lambda_l1, lambda_edge, n_edges, mean,
+                              logvar, nz, dpred, losses, stream);
 }
 
 extern "C" int cape_bce_logits(const float* logits, int64_t n, float label, float scale, float* dlogits, float* loss,

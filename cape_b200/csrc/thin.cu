@@ -54,6 +54,8 @@ __device__ __forceinline__ void thin_gather(const OpView& op, int r, const float
   }
 }
 
+// TANH: the tanh epilogues (b1tanh), compiled only into instantiations of their own (as in conv_wg_kernel)
+template <bool TANH>
 __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ ConvParams p, int KF, int vec4) {
   __shared__ float Bs[TH_ROWS][TH_MAXKF + 1];
   __shared__ __align__(16) float Ws[TH_MAXKF * TH_MAXCOLS];
@@ -139,6 +141,8 @@ __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ C
           acc.z = acc.z > 0.f ? acc.z : p.alpha * acc.z; acc.w = acc.w > 0.f ? acc.w : p.alpha * acc.w;
         } else if (p.act == CAPE_ACT_RELU) {
           acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f);
+        } else if (TANH && p.act == CAPE_ACT_TANH) {
+          acc.x = tanhf(acc.x); acc.y = tanhf(acc.y); acc.z = tanhf(acc.z); acc.w = tanhf(acc.w);
         }
         *reinterpret_cast<float4*>(p.out + oi) = acc;
       } else {
@@ -147,6 +151,10 @@ __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ C
           *reinterpret_cast<float4*>(p.out + oi) =
               make_float4(acc.x * (a.x > 0.f ? 1.f : p.alpha), acc.y * (a.y > 0.f ? 1.f : p.alpha),
                           acc.z * (a.z > 0.f ? 1.f : p.alpha), acc.w * (a.w > 0.f ? 1.f : p.alpha));
+        } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
+          *reinterpret_cast<float4*>(p.out + oi) =
+              make_float4(acc.x * (1.f - a.x * a.x), acc.y * (1.f - a.y * a.y), acc.z * (1.f - a.z * a.z),
+                          acc.w * (1.f - a.w * a.w));
         } else {  // DUALMASK
           *reinterpret_cast<float4*>(p.out + oi) = acc;
           if (p.out2 != nullptr)
@@ -174,9 +182,13 @@ __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ C
       if (p.bias != nullptr) acc += __ldg(p.bias + (p.bias_per_row ? (size_t)r * ncols : 0) + c);
       if (p.act == CAPE_ACT_LEAKY) acc = acc > 0.f ? acc : p.alpha * acc;
       else if (p.act == CAPE_ACT_RELU) acc = fmaxf(acc, 0.f);
+      else if (TANH && p.act == CAPE_ACT_TANH) acc = tanhf(acc);
       p.out[oi] = acc;
     } else if (p.epilogue == CAPE_EPI_SLOPE) {
       p.out[oi] = acc * (__ldg(p.aux + oi) > 0.f ? 1.f : p.alpha);
+    } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
+      const float a = __ldg(p.aux + oi);
+      p.out[oi] = acc * (1.f - a * a);
     } else {  // DUALMASK
       p.out[oi] = acc;
       if (p.out2 != nullptr) p.out2[oi] = __ldg(p.aux + oi) > 0.f ? acc : 0.f;
@@ -392,6 +404,7 @@ __global__ void __launch_bounds__(256) thinout_combine_kernel(const __grid_const
     if (p.bias != nullptr) v += __ldg(p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) + c);
     if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
     else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
+    else if (p.act == CAPE_ACT_TANH) v = tanhf(v);
     p.out[(size_t)R * p.ncols + c] = v;
   }
 }
@@ -417,7 +430,8 @@ int launch_thin_fwd(const cape_topology* t, const ConvParams& p, bool dual, cuda
   }
   const unsigned grid = (unsigned)((p.total_rows + TH_ROWS - 1) / TH_ROWS);
   const int vec4 = (p.ncols % 4 == 0) && p.ovec && (p.bias == nullptr || aligned16(p.bias));
-  thin_fwd_kernel<<<grid, 256, 0, st>>>(p, KF, vec4);
+  if (p.act == CAPE_ACT_TANH || p.epilogue == CAPE_EPI_TANHGRAD) thin_fwd_kernel<true><<<grid, 256, 0, st>>>(p, KF, vec4);
+  else thin_fwd_kernel<false><<<grid, 256, 0, st>>>(p, KF, vec4);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;

@@ -10,10 +10,32 @@ import torch
 
 from . import _lib
 from . import topology as topo
-from ._lib import (ACT_LEAKY, ACT_NONE, ACT_RELU, EPI_AFFINE, EPI_DUALMASK, EPI_LINEAR, EPI_SLOPE, ApplyArgs, ConvArgs,
-                   DwArgs, GemmItem, WPrep, check)
+from ._lib import (ACT_LEAKY, ACT_NONE, ACT_RELU, ACT_TANH, EPI_AFFINE, EPI_DUALMASK, EPI_LINEAR, EPI_SLOPE,
+                   EPI_TANHGRAD, RECON_HUBER, RECON_L1, RECON_L2, ApplyArgs, ConvArgs, DwArgs, GemmItem, WPrep, check)
 
 LEAKY_ALPHA = 0.2  # tf.nn.leaky_relu default (lib/models.py:109,506,582)
+
+# The reference's `--activation` (self.brelu, lib/models.py:60,105-121) as (forward activation of the conv epilogue,
+# data-gradient epilogue given the layer's output, its alpha).  ReLU's backward is the SLOPE mask with alpha 0: aux > 0
+# on the output gives gradient 0 where the output is exactly 0, as tf.nn.relu's gradient does.
+BRELU = {"b1leakyrelu": (ACT_LEAKY, EPI_SLOPE, LEAKY_ALPHA), "b1relu": (ACT_RELU, EPI_SLOPE, 0.0),
+         "b1tanh": (ACT_TANH, EPI_TANHGRAD, 0.0)}
+HUBER_DELTA = 0.1  # tf.losses.huber_loss(delta=0.1), lib/models.py:362-365
+
+
+def recon_kind(loss):
+    """The reconstruction loss of the reference's `--loss` (lib/models.py:357-369): 'l1' absolute difference, 'huber'
+    Huber with delta 0.1, any other string the mean squared error."""
+    return {"l1": RECON_L1, "huber": RECON_HUBER}.get(loss, RECON_L2)
+
+
+def brelu(activation):
+    """BRELU[activation]; the encoder / discriminator activations the reference defines but this port does not build
+    raise here."""
+    if activation not in BRELU:
+        raise NotImplementedError("activation must be one of %s (lib/models.py:105-121); %r is not built"
+                                  % (sorted(BRELU), activation))
+    return BRELU[activation]
 
 # Optional per-launch timing (bench.py's roofline pass): when PROFILE is a list, every helper below brackets its
 # launch with CUDA events on the launching stream and appends (family, tag, algorithmic_bytes, ev0, ev1).

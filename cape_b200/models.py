@@ -28,10 +28,12 @@ class CAPE(object):
                  regularization=0, batch_size=32, seed=123, lambda_recon=1.0, lambda_edge=0.0, lambda_latent=1e-3,
                  restart=False, name="", loss_mask=None, device=0, ref_compat=True, checkpoint_dir="checkpoints",
                  device_dataset=True, **unused):
-        # name-based operator seam of base_model (lib/models.py:58-62): only the shipped choice has kernels
-        if (filter, activation, pool, unpool) != ("chebyshev5", "b1leakyrelu", "poolwT", "poolwT"):
-            raise NotImplementedError("kernels exist for filter='chebyshev5', activation='b1leakyrelu', "
-                                      "pool=unpool='poolwT' (the configuration of every shipped config)")
+        # name-based operator seam of base_model (lib/models.py:58-62): kernels exist for chebyshev5 / poolwT and the
+        # one-bias-per-filter activations
+        if (filter, pool, unpool) != ("chebyshev5", "poolwT", "poolwT"):
+            raise NotImplementedError("kernels exist for filter='chebyshev5' and pool=unpool='poolwT' (the configuration "
+                                      "of every shipped config)")
+        E.brelu(activation)                  # b1leakyrelu, b1relu or b1tanh; anything else raises
         if loss_mask == "binary":
             raise NotImplementedError("loss_mask='binary' is broken in the reference too (lib/models.py:49-50)")
         self.Laplacian, self.Downsample_mtx, self.Upsample_mtx, self.p = L, D, U, p
@@ -56,6 +58,7 @@ class CAPE(object):
                         decay_steps=decay_steps if decay_steps else 1, momentum=momentum, lr_warmup=bool(lr_warmup),
                         optimizer=optimizer, regularization=regularization, lambda_recon=lambda_recon,
                         lambda_edge=lambda_edge, lambda_latent=lambda_latent, lambda_gan=lambda_gan, loss=loss,
+                        activation=activation,
                         batch_size=int(batch_size), seed=seed)
         self.net = None
         self.rng = np.random.RandomState(seed)
@@ -310,9 +313,16 @@ class CAPE(object):
             if labels is not None:
                 gt = self._pad(labels[b:e]).to(net.device)
                 net.losses.zero_()
-                _lib.check(net.tp.lib.cape_recon_losses(net.tp.h, net.nbr_op, E._ptr(net.x_hat), E._ptr(gt), N, net.p[0],
-                                                        0.0, 0.0, net.n_edges, E._ptr(net.z_mean), E._ptr(net.z_logvar),
-                                                        self.nz, E._ptr(net.d_xhat), E._ptr(net.losses), E._stream()))
+                kind = E.recon_kind(self.cfg["loss"])               # the configured loss (models.py:357-369)
+                rest = (net.n_edges, E._ptr(net.z_mean), E._ptr(net.z_logvar), self.nz, E._ptr(net.d_xhat),
+                      E._ptr(net.losses), E._stream())
+                if kind == E.RECON_L1:
+                    rc = net.tp.lib.cape_recon_losses(net.tp.h, net.nbr_op, E._ptr(net.x_hat), E._ptr(gt), N, net.p[0],
+                                                      0.0, 0.0, *rest)
+                else:
+                    rc = net.tp.lib.cape_recon_losses_ex(net.tp.h, net.nbr_op, E._ptr(net.x_hat), E._ptr(gt), N,
+                                                         net.p[0], kind, E.HUBER_DELTA, 0.0, 0.0, *rest)
+                _lib.check(rc)
                 v = net.losses.cpu().numpy()
                 lr_.append(v[0]); le_.append(v[1]); ll_.append(v[2])
         if labels is None:

@@ -17,7 +17,7 @@ import torch
 from . import _lib
 from . import engine as E
 from . import topology as topo
-from .engine import (ACT_LEAKY, ACT_NONE, EPI_AFFINE, EPI_DUALMASK, EPI_LINEAR, EPI_SLOPE, ConvSite, Topology,
+from .engine import (ACT_LEAKY, ACT_NONE, EPI_AFFINE, EPI_DUALMASK, EPI_LINEAR, ConvSite, Topology,
                      act_bwd, axpy, cheb_call, cheb_dw, colsum, gemm)
 from .params import init_params, is_d_param, is_g_param, param_specs
 
@@ -601,11 +601,12 @@ class EncResBlock:
         nm = "enc/res%d" % (i + 1)
         self.conv1 = ChebLayer(net, ConvSite(tp, L, K, order_in=order_in, order_out=order_mid), Fin, C, Fo,
                                w(sc + "filter_1/weights"), g(sc + "filter_1/weights"), bias=w(sc + "bias_relu_1/bias"),
-                               gbias=g(sc + "bias_relu_1/bias"), act=ACT_LEAKY, need_dx=(i > 0), maxN=maxN,
+                               gbias=g(sc + "bias_relu_1/bias"), act=net.brelu[0], need_dx=(i > 0), maxN=maxN,
                                name=nm + "/conv1", fused=True)
         self.conv2 = ChebLayer(net, ConvSite(tp, L, K, D=D, order_in=order_mid, order_out=order_out), Fo, 0, Fo,
                                w(sc + "filter_2/weights"), g(sc + "filter_2/weights"), bias=w(sc + "bias_relu_2/bias"),
-                               gbias=g(sc + "bias_relu_2/bias"), act=ACT_LEAKY, maxN=maxN, name=nm + "/conv2", fused=True)
+                               gbias=g(sc + "bias_relu_2/bias"), act=net.brelu[0], maxN=maxN, name=nm + "/conv2",
+                               fused=True)
         self.skip = ConvSite(tp, L, 1, D=D, order_in=order_in, order_out=order_out)      # x -> D x
         self.proj = None
         if (sc + "1x1-conv/weights") in net.specs:
@@ -638,11 +639,12 @@ class EncResBlock:
         self.conv2.fwd(h1, None, out, extra=[t])
 
     def bwd(self, x, ycat, g2, dx=None, dx_aux=None, dycat=None):
-        """g2: gradient w.r.t. conv2's pre-activation (the block's output rows); dx (written, SLOPE epilogue with the
-        producing block's output dx_aux) when the block has an input gradient; dycat +=."""
+        """g2: gradient w.r.t. conv2's pre-activation (the block's output rows); dx (written, through the activation's
+        backward given the producing block's output dx_aux) when the block has an input gradient; dycat +=."""
         N, sk = g2.shape[0], self.skip
         h1, dh1 = self.h1[:N], self.dh1[:N]
-        self.conv2.bwd(h1, None, g2, dx=dh1, dx_epi=EPI_SLOPE, dx_aux=h1)
+        _, epi, alpha = self.net.brelu
+        self.conv2.bwd(h1, None, g2, dx=dh1, dx_epi=epi, dx_aux=h1, dx_alpha=alpha)
         if self.proj is not None:
             self.proj.bwd(x, ycat, g2, dycat=dycat)             # weight (and condition) gradients of the projection
         if dx is None:
@@ -654,7 +656,7 @@ class EncResBlock:
                      w_stride=self.Fin, wT=p.W3[:, 0, :], wT_stride=self.Fo)
         else:
             t = dict(src=g2, op=sk.opsT[0], F=self.Fo, src_rows=sk.rows_out, src_stride=self.Fo, w=None, w_stride=0)
-        self.conv1.bwd(x, ycat, dh1, dx=dx, dx_epi=EPI_SLOPE, dx_aux=dx_aux, dycat=dycat, dx_extra=[t])
+        self.conv1.bwd(x, ycat, dh1, dx=dx, dx_epi=epi, dx_aux=dx_aux, dx_alpha=alpha, dycat=dycat, dx_extra=[t])
 
 
 class CapeNetwork:
@@ -675,9 +677,11 @@ class CapeNetwork:
         c = self.cfg
         if not c["use_res_block_dec"] or c["reduce_dim"] <= 0:
             raise NotImplementedError("the plain decoder (use_res_block_dec=0) and reduce_dim=0 are not built")
-        if c["optimizer"] not in ("sgd", "adam") or c["loss"] != "l1":
-            raise NotImplementedError("optimizer must be 'sgd' (momentum) or 'adam' (lib/models.py:449-453); only "
-                                      "loss='l1' is implemented")
+        if c["optimizer"] not in ("sgd", "adam"):
+            raise NotImplementedError("optimizer must be 'sgd' (momentum) or 'adam' (lib/models.py:449-453)")
+        # the encoder / discriminator activation (forward act, backward epilogue, alpha) and the reconstruction loss
+        self.brelu = E.brelu(c.get("activation", "b1leakyrelu"))
+        self.recon_kind = E.recon_kind(c["loss"])
         self.adam = c["optimizer"] == "adam"
         self.adam_t = 0                     # optimiser applications so far (TF: beta1_power = beta1 ** (adam_t + 1))
         self.tp = tp = Topology(device)
@@ -739,7 +743,7 @@ class CapeNetwork:
                 site = ConvSite(tp, L[i], K[i], D=D[i], order_in=oi, order_out=og[i + 1])
                 sc = "generator/encoder/encoder_conv%d" % (i + 1)
                 self.enc.append(ChebLayer(self, site, fin, Ci, F[i], w(sc + "/weights"), g(sc + "/weights"),
-                                          bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=ACT_LEAKY, need_dx=(i > 0),
+                                          bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=self.brelu[0], need_dx=(i > 0),
                                           maxN=N, name="enc/conv%d" % (i + 1)))
             fin = F[i]
         red = specs["generator/encoder/1x1-conv/weights"][1]
@@ -784,7 +788,7 @@ class CapeNetwork:
             site = ConvSite(tp, L_d[i], Kd, D=D_d[i], order_in=od[i] if i > 0 else None, order_out=od[i + 1])
             sc = "discriminator/shared/conv%d" % (i + 1)
             self.disc.append(ChebLayer(self, site, fin, Cc if i == 0 else 0, F[i], w(sc + "/weights"),
-                                       g(sc + "/weights"), bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=ACT_LEAKY,
+                                       g(sc + "/weights"), bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=self.brelu[0],
                                        maxN=2 * N, n_cs_slots=2, name="disc/conv%d" % (i + 1)))
             fin = F[i]
         self.disc_pred = ChebLayer(self, ConvSite(tp, L_d[-1], K[-1], order_in=od[-1], order_out=od[-1]), fin, 0, 1,
@@ -1034,10 +1038,11 @@ class CapeNetwork:
         acts = [a[lo:hi] for a in self.disc_act]
         gs = [gb[: hi - lo] for gb in self.g_disc]
         yc = self.ycat[lo:hi]
-        self.disc_pred.bwd(acts[-1], None, dlogits, dx=gs[-1], dx_epi=EPI_SLOPE, dx_aux=acts[-1], want_dw=want_dw,
-                           cs_slot=cs_slot)
+        _, epi, alpha = self.brelu
+        self.disc_pred.bwd(acts[-1], None, dlogits, dx=gs[-1], dx_epi=epi, dx_aux=acts[-1], dx_alpha=alpha,
+                           want_dw=want_dw, cs_slot=cs_slot)
         for i in range(n - 1, 0, -1):
-            self.disc[i].bwd(acts[i - 1], None, gs[i], dx=gs[i - 1], dx_epi=EPI_SLOPE, dx_aux=acts[i - 1],
+            self.disc[i].bwd(acts[i - 1], None, gs[i], dx=gs[i - 1], dx_epi=epi, dx_aux=acts[i - 1], dx_alpha=alpha,
                              want_dw=want_dw, cs_slot=cs_slot)
         self.disc[0].bwd(self.xcat[lo:hi], yc, gs[0], dx=dx, dycat=dycat, want_dw=want_dw, cs_slot=cs_slot)
 
@@ -1082,8 +1087,9 @@ class CapeNetwork:
         self.fc_var.bwd(flat, self.z_logvar, self.g_logvar, dx=gflat, dx_beta=1.0)
         self._fc_reg(("generator/encoder/fc_mean", "generator/encoder/fc_var"))
         self._reduce_bucket("enc_fc")                       # 28 MB of gradients are final: all-reduce behind the conv backward
-        self.enc_1x1.bwd(self.enc_act[-1], None, self.g_enc_red, dx=self.g_enc[-1], dx_epi=EPI_SLOPE,
-                         dx_aux=self.enc_act[-1])
+        _, epi, alpha = self.brelu
+        self.enc_1x1.bwd(self.enc_act[-1], None, self.g_enc_red, dx=self.g_enc[-1], dx_epi=epi,
+                         dx_aux=self.enc_act[-1], dx_alpha=alpha)
         yc = self.ycat_g if self.cond_enc else None
         dyc = self.d_ycat if self.cond_enc else None        # complete before cond_bwd (the small products flush first)
         for i in range(len(self.enc) - 1, 0, -1):
@@ -1091,8 +1097,8 @@ class CapeNetwork:
                 self.enc[i].bwd(self.enc_act[i - 1], None, self.g_enc[i], dx=self.g_enc[i - 1],
                                 dx_aux=self.enc_act[i - 1])
             else:
-                self.enc[i].bwd(self.enc_act[i - 1], None, self.g_enc[i], dx=self.g_enc[i - 1], dx_epi=EPI_SLOPE,
-                                dx_aux=self.enc_act[i - 1])
+                self.enc[i].bwd(self.enc_act[i - 1], None, self.g_enc[i], dx=self.g_enc[i - 1], dx_epi=epi,
+                                dx_aux=self.enc_act[i - 1], dx_alpha=alpha)
         self.enc[0].bwd(self.in_x, yc, self.g_enc[0], dycat=dyc)
 
     def cond_bwd(self):
@@ -1166,10 +1172,10 @@ class CapeNetwork:
         # gradient buffers the discriminator's weight gradients are still reading on the side stream: join first)
         self.join_dw()
         self.disc_bwd(N, 2 * N, self.d_logits_g, want_dw=False, dx=self.d_xhat, dycat=self.d_ycat, cs_slot=1)
-        _lib.check(lib.cape_recon_losses(tp.h, self.nbr_op, E._ptr(self.x_hat), E._ptr(self.in_x), N, self.p[0],
-                                         float(c["lambda_recon"]), float(c["lambda_edge"]), self.n_edges,
-                                         E._ptr(self.z_mean), E._ptr(self.z_logvar), self.nz, E._ptr(self.d_xhat),
-                                         E._ptr(L), st()))
+        _lib.check(lib.cape_recon_losses_ex(tp.h, self.nbr_op, E._ptr(self.x_hat), E._ptr(self.in_x), N, self.p[0],
+                                            self.recon_kind, E.HUBER_DELTA, float(c["lambda_recon"]),
+                                            float(c["lambda_edge"]), self.n_edges, E._ptr(self.z_mean),
+                                            E._ptr(self.z_logvar), self.nz, E._ptr(self.d_xhat), E._ptr(L), st()))
         self.decoder_bwd()
         self._fc_reg(("generator/decoder/fc1",))
         if not self.side_glue:

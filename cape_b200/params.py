@@ -9,7 +9,7 @@ DEFAULTS = dict(
     # architecture (main.py:35-40,60-70; config_parser.py defaults)
     F=[64, 64, 128, 128, 256, 256, 512, 512], K=[2] * 8, Kd=3, nz=18, nz_cond=24, nz_cond2=8,
     cond_dim=126, cond2_dim=4, n_layer_cond=1, reduce_dim=64, affine=False, nn_input_channel=3,
-    use_res_block=False, use_res_block_dec=True, cond_encoder=False, optim_condnet=True,
+    use_res_block=False, use_res_block_dec=True, cond_encoder=False, optim_condnet=True, activation="b1leakyrelu",
     # optimisation / loss (config_parser.py:27-46)
     lr=8e-3, lr_scaler=0.1, decay_rate=0.99, decay_steps=1, momentum=0.9, lr_warmup=False, optimizer="sgd",
     regularization=2e-3, lambda_recon=1.0, lambda_edge=1.0, lambda_latent=8e-4, lambda_gan=0.1, loss="l1",

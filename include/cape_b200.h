@@ -93,9 +93,12 @@ enum {
   CAPE_EPI_LINEAR = 0,   /* out = act(acc0 + bias)                       chebyshev5 + b1leakyrelu, models.py:69-109 */
   CAPE_EPI_AFFINE = 1,   /* out = acc1 + relu(acc0); out2 = relu(acc0)   res_block_affine, models.py:776-793 */
   CAPE_EPI_SLOPE = 2,    /* out = acc0 * (aux > 0 ? 1 : alpha)           backward through (leaky-)ReLU given its output */
-  CAPE_EPI_DUALMASK = 3  /* out = acc0; out2 = acc0 * (aux > 0)          backward into an affine block's output */
+  CAPE_EPI_DUALMASK = 3, /* out = acc0; out2 = acc0 * (aux > 0)          backward into an affine block's output */
+  CAPE_EPI_TANHGRAD = 4  /* out = acc0 * (1 - aux^2)                     backward through tanh given its output
+                          * (b1tanh, models.py:111-115); ReLU (b1relu, :117-121) is SLOPE with alpha = 0 */
 };
-enum { CAPE_ACT_NONE = 0, CAPE_ACT_LEAKY = 1, CAPE_ACT_RELU = 2 };
+/* LEAKY: b1leakyrelu (models.py:105-109), RELU: b1relu (:117-121), TANH: b1tanh (:111-115, the precise tanhf) */
+enum { CAPE_ACT_NONE = 0, CAPE_ACT_LEAKY = 1, CAPE_ACT_RELU = 2, CAPE_ACT_TANH = 3 };
 
 typedef struct {
   int N, rows_out, ncols;
@@ -108,7 +111,7 @@ typedef struct {
   float alpha;         /* negative slope (LEAKY: 0.2 = tf.nn.leaky_relu default; SLOPE epilogue) */
   const float* bias;   /* [ncols] or [rows_out, ncols] (NULL: none) */
   int bias_per_row;    /* 1: per-vertex bias (decoder outputs, models.py:615) */
-  const float* aux;    /* [N, rows_out, ncols] (SLOPE / DUALMASK) */
+  const float* aux;    /* [N, rows_out, ncols] (SLOPE / DUALMASK / TANHGRAD) */
   float* out;          /* [N, rows_out, ncols] */
   float* out2;         /* [N, rows_out, ncols] or NULL */
   /* 1: fail (rc < 0) instead of falling back to the gather / fp32-pipe kernels when the plain-operand tensor-core kernel
@@ -146,7 +149,7 @@ typedef struct {
   float alpha;
   const float* bias;   /* [ncols] or [rows_out, ncols] */
   int bias_per_row;
-  const float* aux;    /* [N, rows_out, ncols] (SLOPE / DUALMASK) */
+  const float* aux;    /* [N, rows_out, ncols] (SLOPE / DUALMASK / TANHGRAD) */
   float* out;          /* rows out_stride floats apart (0: ncols) -- the result may land inside a wider buffer */
   int out_stride;
   float* out2;         /* same stride, or NULL */
@@ -269,7 +272,7 @@ int cape_gather_rows(const float* src, int64_t row_floats, int n_src, const int3
                      void* stream);
 
 /* ---- losses (CAPE.loss, lib/models.py:354-416; losses.edge_loss_calc, lib/losses.py:9-25) ----------
- * Reconstruction L1 (mean |pred-gt|), edge loss (mean over edges of ||(p_a-p_b)-(g_a-g_b)||_2; the
+ * Reconstruction L1 (mean |pred-gt|; cape_recon_losses_ex below: L2 / Huber), edge loss (mean over edges of ||(p_a-p_b)-(g_a-g_b)||_2; the
  * template added at models.py:375 cancels), KL (mean_n -0.5*sum(1+lv-mu^2-e^lv)); writes
  * losses[0..2] = {recon, edge, kl} (unweighted) and ACCUMULATES lambda-weighted gradients into dpred.
  * nbr_op: id of the level-0 adjacency operator (its idx table lists each vertex's neighbours). */
@@ -277,6 +280,17 @@ int cape_recon_losses(cape_topology* t, int nbr_op, const float* pred, const flo
                       float lambda_l1, float lambda_edge, int n_edges,
                       const float* mean, const float* logvar, int nz,
                       float* dpred, float* losses, void* stream);
+/* The reconstruction term of the reference's `--loss` switch (models.py:357-369, every one Reduction.MEAN over the
+ * N*rows*3 coordinates d = pred - gt, weights 1):
+ *   CAPE_RECON_L1     mean |d|                                   (absolute_difference)   gradient sign(d) / cnt
+ *   CAPE_RECON_L2     mean d^2                                   (mean_squared_error)    gradient 2 d / cnt
+ *   CAPE_RECON_HUBER  mean 0.5 q^2 + delta (|d| - q), q = min(|d|, delta)   (huber_loss) gradient clamp(d, +-delta) / cnt
+ * losses[0] is that term, scaled into dpred by lambda_recon; the edge and KL terms are cape_recon_losses'.
+ * cape_recon_losses is kind CAPE_RECON_L1 of this call (bit-identical results).  delta is read by HUBER only (> 0). */
+enum { CAPE_RECON_L1 = 0, CAPE_RECON_L2 = 1, CAPE_RECON_HUBER = 2 };
+int cape_recon_losses_ex(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
+                         int kind, float delta, float lambda_recon, float lambda_edge, int n_edges,
+                         const float* mean, const float* logvar, int nz, float* dpred, float* losses, void* stream);
 /* Sigmoid cross-entropy with a constant label (tf.nn.sigmoid_cross_entropy_with_logits, models.py:387-389):
  * loss[0] += mean(bce(logits, label)); dlogits = scale * d mean(bce)/dlogits  */
 int cape_bce_logits(const float* logits, int64_t n, float label, float scale, float* dlogits, float* loss,

@@ -41,21 +41,12 @@ struct ApParams {
   int slot_ws[CAPE_MAX_TERMS];
   const float* cond;
   int C;
-  int epilogue, act;
-  float alpha;
-  const float* bias;
-  int bias_per_row;
-  const float* aux;
-  float* out;
-  float* out2;
+  EpiParams epi;
   int out_stride;
   long long term_stride;               // > 0: "separate" mode, term t is written on its own to out + t * term_stride
 };
 
 __device__ __forceinline__ float4 f4_zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
-__device__ __forceinline__ void f4_axpy(float4& a, float s, const float4& x) {
-  a.x = fmaf(s, x.x, a.x); a.y = fmaf(s, x.y, a.y); a.z = fmaf(s, x.z, a.z); a.w = fmaf(s, x.w, a.w);
-}
 
 __device__ __forceinline__ void ap_advance(int& r, int& n, int by, int rows) {
   r += by;
@@ -64,47 +55,24 @@ __device__ __forceinline__ void ap_advance(int& r, int& n, int by, int rows) {
 
 template <bool DUAL, bool TANH>
 __device__ __forceinline__ void ap_store(const ApParams& p, long long R, int r, int c, float4 a0, float4 a1) {
+  const EpiParams& e = p.epi;
   const size_t o = (size_t)R * p.out_stride + c;
-  float v0[4] = {a0.x, a0.y, a0.z, a0.w}, v1[4] = {a1.x, a1.y, a1.z, a1.w}, o1[4], o2[4];
-  bool write2 = false;
-  if (p.epilogue == CAPE_EPI_LINEAR) {
+  float v0[4] = {a0.x, a0.y, a0.z, a0.w}, v1[4] = {0.f, 0.f, 0.f, 0.f}, b[4] = {0.f, 0.f, 0.f, 0.f};
+  float ax[4] = {0.f, 0.f, 0.f, 0.f}, o1[4], o2[4];
+  if (DUAL) { v1[0] = a1.x; v1[1] = a1.y; v1[2] = a1.z; v1[3] = a1.w; }
+  if (e.epilogue == CAPE_EPI_LINEAR && e.bias != nullptr) {
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float v = v0[j];
-      if (p.bias != nullptr) v += __ldg(p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) + c + j);
-      if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
-      else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
-      else if (TANH && p.act == CAPE_ACT_TANH) v = tanhf(v);
-      o1[j] = v;
-    }
-  } else if (p.epilogue == CAPE_EPI_AFFINE) {
-    write2 = p.out2 != nullptr;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float rg = fmaxf(v0[j], 0.f);
-      o1[j] = (DUAL ? v1[j] : 0.f) + rg;
-      o2[j] = rg;
-    }
-  } else {
-    const float4 ax = ldg4(p.aux + (size_t)R * p.ncols + c);
-    const float a[4] = {ax.x, ax.y, ax.z, ax.w};
-    if (p.epilogue == CAPE_EPI_SLOPE) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (a[j] > 0.f ? 1.f : p.alpha);
-    } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
-#pragma unroll
-      for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (1.f - a[j] * a[j]);
-    } else {
-      write2 = p.out2 != nullptr;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) { o1[j] = v0[j]; o2[j] = a[j] > 0.f ? v0[j] : 0.f; }
-    }
+    for (int j = 0; j < 4; ++j) b[j] = __ldg(e.bias + (e.bias_per_row ? (size_t)r * p.ncols : 0) + c + j);
+  } else if (epi_reads_aux(e.epilogue)) {
+    const float4 a4 = ldg4(e.aux + (size_t)R * p.ncols + c);
+    ax[0] = a4.x; ax[1] = a4.y; ax[2] = a4.z; ax[3] = a4.w;
   }
-  *reinterpret_cast<float4*>(p.out + o) = make_float4(o1[0], o1[1], o1[2], o1[3]);
-  if (write2) *reinterpret_cast<float4*>(p.out2 + o) = make_float4(o2[0], o2[1], o2[2], o2[3]);
+  const bool write2 = apply_epilogue<TANH>(e, v0, v1, b, ax, o1, o2);
+  *reinterpret_cast<float4*>(e.out + o) = make_float4(o1[0], o1[1], o1[2], o1[3]);
+  if (write2) *reinterpret_cast<float4*>(e.out2 + o) = make_float4(o2[0], o2[1], o2[2], o2[3]);
 }
 
-// TANH: the tanh epilogues (b1tanh), compiled only into instantiations of their own (as in conv_wg_kernel)
+// TANH: the tanh epilogues (needs_tanh)
 template <bool DUAL, bool TANH>
 __global__ void __launch_bounds__(AP_THREADS, 3) apply_kernel(const __grid_constant__ ApParams p) {
   __shared__ __align__(16) float qs[AP_QS];
@@ -112,18 +80,10 @@ __global__ void __launch_bounds__(AP_THREADS, 3) apply_kernel(const __grid_const
   const long long R0 = (long long)blockIdx.x * AP_R;
   const int n_first = (int)(R0 / p.rows_out);
   if (p.nslots > 0) {
-    // condition vectors of the samples this CTA touches: q[s][slot][c] = cond[n_first + s, :] @ wc_slot[:, c]
+    // condition vectors of the samples this CTA touches
     const long long rlast = min(p.total_rows, R0 + AP_R) - 1;
     const int S = (int)(rlast / p.rows_out) - n_first + 1;
-    const int total = S * p.nslots * p.ncols;
-    for (int o = threadIdx.x; o < total; o += AP_THREADS) {
-      const int c = o % p.ncols, slot = (o / p.ncols) % p.nslots, s = o / (p.ncols * p.nslots);
-      const float* y = p.cond + (size_t)(n_first + s) * p.C;
-      const float* wc = p.slot_w[slot] + c;
-      float q = 0.f;
-      for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * p.slot_ws[slot]), q);
-      qs[o] = q;
-    }
+    stage_cond<4>(p, qs, n_first, S, 0, p.ncols, p.ncols, threadIdx.x, AP_THREADS);
     __syncthreads();
   }
   const int lr = threadIdx.x / p.tpr, c = (threadIdx.x % p.tpr) * 4;
@@ -151,15 +111,15 @@ __global__ void __launch_bounds__(AP_THREADS, 3) apply_kernel(const __grid_const
         ell_gather4_pair(tm.op, ra, rb, pa, pb, (size_t)tm.src_stride, ta, tb);
       }
       if (tm.slot >= 0) {
-        const float ca = tm.op.rowsum ? __ldg(tm.op.rowsum + ra) : 1.f, cb = tm.op.rowsum ? __ldg(tm.op.rowsum + rb) : 1.f;
-        const float4 qa = *reinterpret_cast<const float4*>(qs + ((size_t)(na - n_first) * p.nslots + tm.slot) * p.ncols + c);
-        const float4 qb = *reinterpret_cast<const float4*>(qs + ((size_t)(nb - n_first) * p.nslots + tm.slot) * p.ncols + c);
-        f4_axpy(ta, ca, qa);
-        f4_axpy(tb, cb, qb);
+        const float ca = cond_coef(tm.op, ra), cb = cond_coef(tm.op, rb);
+        const float4 qa = *reinterpret_cast<const float4*>(cond_vec(qs, na - n_first, tm.slot, p.nslots, p.ncols) + c);
+        const float4 qb = *reinterpret_cast<const float4*>(cond_vec(qs, nb - n_first, tm.slot, p.nslots, p.ncols) + c);
+        fma4(ta, ca, qa);
+        fma4(tb, cb, qb);
       }
       if (p.term_stride > 0) {
         // separate mode (the K basis tensors of a layer in one launch): no summation, no epilogue
-        float* o = p.out + (size_t)t * p.term_stride;
+        float* o = p.epi.out + (size_t)t * p.term_stride;
         *reinterpret_cast<float4*>(o + (size_t)Ra * p.out_stride + c) =
             make_float4(tm.scale * ta.x, tm.scale * ta.y, tm.scale * ta.z, tm.scale * ta.w);
         if (vb)
@@ -167,8 +127,8 @@ __global__ void __launch_bounds__(AP_THREADS, 3) apply_kernel(const __grid_const
               make_float4(tm.scale * tb.x, tm.scale * tb.y, tm.scale * tb.z, tm.scale * tb.w);
         continue;
       }
-      if (DUAL && tm.acc == 1) { f4_axpy(a1, tm.scale, ta); f4_axpy(b1, tm.scale, tb); }
-      else { f4_axpy(a0, tm.scale, ta); f4_axpy(b0, tm.scale, tb); }
+      if (DUAL && tm.acc == 1) { fma4(a1, tm.scale, ta); fma4(b1, tm.scale, tb); }
+      else { fma4(a0, tm.scale, ta); fma4(b0, tm.scale, tb); }
     }
     if (p.term_stride > 0) continue;
     ap_store<DUAL, TANH>(p, Ra, ra, c, a0, a1);
@@ -188,8 +148,6 @@ extern "C" int cape_apply(cape_topology* t, const cape_apply_args* a, void* stre
   CAPE_REQUIRE(a->nterms >= 1 && a->nterms <= CAPE_MAX_TERMS, "nterms out of range");
   CAPE_REQUIRE(a->out != nullptr, "out is null");
   CAPE_REQUIRE(a->ncols % 4 == 0 && a->ncols <= 4 * AP_THREADS, "cape_apply needs ncols % 4 == 0 and ncols <= 1024");
-  CAPE_REQUIRE(a->epilogue >= CAPE_EPI_LINEAR && a->epilogue <= CAPE_EPI_TANHGRAD, "unknown epilogue");
-  CAPE_REQUIRE(a->act >= CAPE_ACT_NONE && a->act <= CAPE_ACT_TANH, "unknown activation");
   ApParams p{};
   p.N = a->N; p.rows_out = a->rows_out; p.ncols = a->ncols; p.nterms = a->nterms;
   p.total_rows = (long long)a->N * a->rows_out;
@@ -218,28 +176,24 @@ extern "C" int cape_apply(cape_topology* t, const cape_apply_args* a, void* stre
       p.slot_w[p.nslots] = s.wc; p.slot_ws[p.nslots] = s.wc_stride; ++p.nslots;
     }
   }
-  if (p.nslots > 0) {
-    const long long max_samples = (p.rows_cta - 1) / a->rows_out + 2;
-    CAPE_REQUIRE(max_samples * p.nslots * a->ncols <= AP_QS, "too many condition columns for the staging buffer");
-  }
+  CAPE_REQUIRE(max_tile_samples(p.rows_cta, a->rows_out) * p.nslots * a->ncols <= AP_QS,
+               "too many condition columns for the staging buffer");
   p.cond = a->cond; p.C = a->C;
-  p.epilogue = a->epilogue; p.act = a->act; p.alpha = a->alpha;
-  p.bias = a->bias; p.bias_per_row = a->bias_per_row; p.aux = a->aux;
-  p.out = a->out; p.out2 = a->out2;
+  if (fill_epilogue(a, dual, &p.epi) != 0) return -1;
   p.term_stride = a->term_stride;
   if (a->term_stride != 0) {
     CAPE_REQUIRE(a->term_stride > 0 && a->term_stride % 4 == 0 && a->epilogue == CAPE_EPI_LINEAR && !a->bias &&
                  a->act == CAPE_ACT_NONE && p.nslots == 0 && !dual,
                  "separate outputs (term_stride) take plain terms: LINEAR epilogue, no bias / activation / condition");
   }
-  if (a->epilogue == CAPE_EPI_SLOPE || a->epilogue == CAPE_EPI_DUALMASK || a->epilogue == CAPE_EPI_TANHGRAD) {
-    CAPE_REQUIRE(a->aux && aligned16(a->aux), "epilogue needs a 16-byte aligned aux");
+  if (epi_reads_aux(a->epilogue)) {
+    CAPE_REQUIRE(aligned16(a->aux), "epilogue needs a 16-byte aligned aux");
     CAPE_REQUIRE(p.out_stride == a->ncols, "SLOPE / DUALMASK / TANHGRAD epilogues need out_stride == ncols");
   }
   const long long blocks = (p.total_rows + p.rows_cta - 1) / p.rows_cta;
   CAPE_REQUIRE(blocks < (1LL << 31), "grid too large");
   cudaStream_t st = (cudaStream_t)stream;
-  const bool tanh = a->act == CAPE_ACT_TANH || a->epilogue == CAPE_EPI_TANHGRAD;
+  const bool tanh = needs_tanh(p.epi);
   if (dual) {
     if (tanh) apply_kernel<true, true><<<(unsigned)blocks, AP_THREADS, 0, st>>>(p);
     else apply_kernel<true, false><<<(unsigned)blocks, AP_THREADS, 0, st>>>(p);

@@ -86,6 +86,19 @@ __device__ __forceinline__ void fma4(float4& a, float s, const float4& x) {
   a.x = fmaf(s, x.x, a.x); a.y = fmaf(s, x.y, a.y); a.z = fmaf(s, x.z, a.z); a.w = fmaf(s, x.w, a.w);
 }
 
+// sum_j w[r, j] * base[idx[r, j] * stride], tap by tap in table order: one scalar column
+__device__ __forceinline__ float ell_gather1(const OpView& op, int r, const float* base, size_t stride) {
+  const int32_t* ip = op.idx + (size_t)r * op.width;
+  const float* wp = op.w + (size_t)r * op.width;
+  float v = 0.f;
+  for (int j = 0; j < op.width; ++j) {
+    const int id = __ldg(ip + j);
+    if (id < 0) break;
+    v = fmaf(__ldg(wp + j), __ldg(base + (size_t)id * stride), v);
+  }
+  return v;
+}
+
 // v += sum_j w[r, j] * src_row(idx[r, j])  for one float4 column group.  Taps are fetched four at a time (the
 // tables are padded to a multiple of 4, empty slots idx = -1 / w = 0) so that four independent neighbour-row loads
 // are in flight per batch instead of one dependent load per tap.

@@ -42,17 +42,8 @@ __device__ __forceinline__ void gather_A(const TermDev& tm, int f0, const int* s
       float v = 0.f;
       if (n >= 0 && f < tm.F) {
         const float* base = tm.src + (size_t)n * tm.src_rows * tm.src_stride + f;
-        if (tm.op.idx == nullptr) {
-          v = __ldg(base + (size_t)r * tm.src_stride);
-        } else {
-          const int32_t* ip = tm.op.idx + (size_t)r * tm.op.width;
-          const float* wp = tm.op.w + (size_t)r * tm.op.width;
-          for (int j = 0; j < tm.op.width; ++j) {
-            const int id = __ldg(ip + j);
-            if (id < 0) break;
-            v = fmaf(__ldg(wp + j), __ldg(base + (size_t)id * tm.src_stride), v);
-          }
-        }
+        if (tm.op.idx == nullptr) v = __ldg(base + (size_t)r * tm.src_stride);
+        else v = ell_gather1(tm.op, r, base, (size_t)tm.src_stride);
       }
       ra[i] = v;
     }
@@ -214,32 +205,19 @@ __global__ void __launch_bounds__(NT, DUAL ? 1 : 2) ellconv_kernel(const __grid_
     t = nt; f0 = nf0;
   }
 
-  // ---- condition broadcast: q[s][slot][c] = cond[n0+s, :] @ Wc_slot[:, col0+c], staged in As -------
+  // ---- condition broadcast, staged in As ---------------------------------------------------------
   float* qs = As;
   const int n_first = s_n[0];
   if (p.nslots > 0) {
     int n_last = n_first;
     for (int i = BM - 1; i > 0; --i)
       if (s_n[i] >= 0) { n_last = s_n[i]; break; }
-    const int S = n_last - n_first + 1;
-    const int total = S * p.nslots * BN;
-    for (int o = tid; o < total; o += NT) {
-      const int c = o % BN;
-      const int slot = (o / BN) % p.nslots;
-      const int s = o / (BN * p.nslots);
-      float q = 0.f;
-      if (col0 + c < p.ncols) {
-        const float* y = p.cond + (size_t)(n_first + s) * p.C;
-        const float* wc = p.slot_w[slot] + col0 + c;
-        const int ws = p.slot_acc[slot] ? p.terms[p.slot_term[slot]].w2_stride : p.terms[p.slot_term[slot]].w_stride;
-        for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * ws), q);
-      }
-      qs[o] = q;
-    }
+    stage_cond<16>(p, qs, n_first, n_last - n_first + 1, col0, BN, p.ncols, tid, NT);
     __syncthreads();
   }
 
-  // ---- epilogue -----------------------------------------------------------------------------------
+  // ---- epilogue (the tanh ones compiled out with two accumulators: refused by cape_cheb_fwd) ----------
+  const EpiParams& e = p.epi;
 #pragma unroll
   for (int i = 0; i < RPT; ++i) {
     const int row = ty + TY * i;
@@ -250,9 +228,8 @@ __global__ void __launch_bounds__(NT, DUAL ? 1 : 2) ellconv_kernel(const __grid_
 #pragma unroll
     for (int j = 0; j < 4; ++j) { v0[j] = acc0[i][j]; v1[j] = DUAL ? acc1[i][j] : 0.f; }
     for (int slot = 0; slot < p.nslots; ++slot) {
-      const TermDev& tm = p.terms[p.slot_term[slot]];
-      const float coef = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
-      const float* q = qs + ((size_t)(n - n_first) * p.nslots + slot) * BN + tx * 4;
+      const float coef = cond_coef(p.terms[p.slot_term[slot]].op, r);
+      const float* q = cond_vec(qs, n - n_first, slot, p.nslots, BN) + tx * 4;
       if (p.slot_acc[slot] == 0) {
 #pragma unroll
         for (int j = 0; j < 4; ++j) v0[j] = fmaf(coef, q[j], v0[j]);
@@ -272,59 +249,32 @@ __global__ void __launch_bounds__(NT, DUAL ? 1 : 2) ellconv_kernel(const __grid_
       }
     }
     const size_t obase = ((size_t)(row0 + row)) * p.ncols + c0;
-    float o1[4], o2[4];
-    bool write2 = false;
-    if (p.epilogue == CAPE_EPI_LINEAR) {
+    float b[4] = {0.f, 0.f, 0.f, 0.f}, ax[4] = {0.f, 0.f, 0.f, 0.f}, o1[4], o2[4];
+    if (e.epilogue == CAPE_EPI_LINEAR && e.bias != nullptr) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float v = v0[j];
-        if (p.bias != nullptr && c0 + j < p.ncols)
-          v += __ldg(p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) + c0 + j);
-        if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
-        else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
-        else if (!DUAL && p.act == CAPE_ACT_TANH) v = tanhf(v);   // DUAL: refused by cape_cheb_fwd
-        o1[j] = v;
-      }
-    } else if (p.epilogue == CAPE_EPI_AFFINE) {
-      write2 = p.out2 != nullptr;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float rg = fmaxf(v0[j], 0.f);
-        o1[j] = v1[j] + rg;
-        o2[j] = rg;
-      }
-    } else {
-      float ax[4];
+      for (int j = 0; j < 4; ++j)
+        if (c0 + j < p.ncols) b[j] = __ldg(e.bias + (e.bias_per_row ? (size_t)r * p.ncols : 0) + c0 + j);
+    } else if (epi_reads_aux(e.epilogue)) {
       if (p.ovec && c0 < p.ncols) {
-        const float4 a4 = ldg4(p.aux + obase);
+        const float4 a4 = ldg4(e.aux + obase);
         ax[0] = a4.x; ax[1] = a4.y; ax[2] = a4.z; ax[3] = a4.w;
       } else {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) ax[j] = (c0 + j < p.ncols) ? __ldg(p.aux + obase + j) : 0.f;
-      }
-      if (p.epilogue == CAPE_EPI_SLOPE) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (ax[j] > 0.f ? 1.f : p.alpha);
-      } else if (!DUAL && p.epilogue == CAPE_EPI_TANHGRAD) {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) o1[j] = v0[j] * (1.f - ax[j] * ax[j]);
-      } else {  // DUALMASK
-        write2 = p.out2 != nullptr;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { o1[j] = v0[j]; o2[j] = ax[j] > 0.f ? v0[j] : 0.f; }
+        for (int j = 0; j < 4; ++j) ax[j] = (c0 + j < p.ncols) ? __ldg(e.aux + obase + j) : 0.f;
       }
     }
+    const bool write2 = apply_epilogue<!DUAL>(e, v0, v1, b, ax, o1, o2);
     if (p.ovec) {
       if (c0 < p.ncols) {
-        *reinterpret_cast<float4*>(p.out + obase) = make_float4(o1[0], o1[1], o1[2], o1[3]);
-        if (write2) *reinterpret_cast<float4*>(p.out2 + obase) = make_float4(o2[0], o2[1], o2[2], o2[3]);
+        *reinterpret_cast<float4*>(e.out + obase) = make_float4(o1[0], o1[1], o1[2], o1[3]);
+        if (write2) *reinterpret_cast<float4*>(e.out2 + obase) = make_float4(o2[0], o2[1], o2[2], o2[3]);
       }
     } else {
 #pragma unroll
       for (int j = 0; j < 4; ++j)
         if (c0 + j < p.ncols) {
-          p.out[obase + j] = o1[j];
-          if (write2) p.out2[obase + j] = o2[j];
+          e.out[obase + j] = o1[j];
+          if (write2) e.out2[obase + j] = o2[j];
         }
     }
   }
@@ -378,17 +328,8 @@ __device__ __forceinline__ void dw_gather(const DwParams& p, long long rbase, lo
       if (R < rend && f < p.F) {
         const int n = (int)(R / p.rows_out), r = (int)(R % p.rows_out);
         const float* base = p.src + (size_t)n * p.src_rows * p.src_stride + f;
-        if (p.op.idx == nullptr) {
-          v = __ldg(base + (size_t)r * p.src_stride);
-        } else {
-          const int32_t* ip = p.op.idx + (size_t)r * p.op.width;
-          const float* wp = p.op.w + (size_t)r * p.op.width;
-          for (int j = 0; j < p.op.width; ++j) {
-            const int id = __ldg(ip + j);
-            if (id < 0) break;
-            v = fmaf(__ldg(wp + j), __ldg(base + (size_t)id * p.src_stride), v);
-          }
-        }
+        if (p.op.idx == nullptr) v = __ldg(base + (size_t)r * p.src_stride);
+        else v = ell_gather1(p.op, r, base, (size_t)p.src_stride);
       }
       ra[i] = v;
     }
@@ -633,23 +574,11 @@ __global__ void __launch_bounds__(256) resample_kernel(OpView op, const float* _
     }
   } else {
     for (int f = lane; f < F; f += 32) {
-      float v = 0.f;
-      if (op.idx == nullptr) {
-        v = __ldg(base + (size_t)r * xs + f);
-      } else {
-        const int32_t* ip = op.idx + (size_t)r * op.width;
-        const float* wp = op.w + (size_t)r * op.width;
-        for (int j = 0; j < op.width; ++j) {
-          const int id = __ldg(ip + j);
-          if (id < 0) break;
-          v = fmaf(__ldg(wp + j), __ldg(base + (size_t)id * xs + f), v);
-        }
-      }
-      out[f] = v;
+      out[f] = op.idx == nullptr ? __ldg(base + (size_t)r * xs + f) : ell_gather1(op, r, base + f, (size_t)xs);
     }
   }
   if (cond != nullptr) {
-    const float coef = op.rowsum ? __ldg(op.rowsum + r) : 1.f;
+    const float coef = cond_coef(op, r);
     for (int c = lane; c < C; c += 32) out[F + c] = coef * __ldg(cond + (size_t)n * C + c);
   }
 }
@@ -731,29 +660,22 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
     }
     if (s.wc) {
       CAPE_REQUIRE(a->cond && a->C > 0, "condition weights without cond");
-      p.slot_term[p.nslots] = ti; p.slot_acc[p.nslots] = 0; p.slot_w[p.nslots] = s.wc; ++p.nslots;
+      p.slot_term[p.nslots] = ti; p.slot_acc[p.nslots] = 0;
+      p.slot_w[p.nslots] = s.wc; p.slot_ws[p.nslots] = s.w_stride; ++p.nslots;
     }
     if (s.wc2) {
       CAPE_REQUIRE(a->cond && a->C > 0 && s.w2, "wc2 needs cond and w2");
-      p.slot_term[p.nslots] = ti; p.slot_acc[p.nslots] = 1; p.slot_w[p.nslots] = s.wc2; ++p.nslots;
+      p.slot_term[p.nslots] = ti; p.slot_acc[p.nslots] = 1;
+      p.slot_w[p.nslots] = s.wc2; p.slot_ws[p.nslots] = s.w2_stride; ++p.nslots;
     }
   }
   p.cond = a->cond; p.C = a->C;
-  p.epilogue = a->epilogue; p.act = a->act; p.alpha = a->alpha;
-  p.bias = a->bias; p.bias_per_row = a->bias_per_row;
-  p.aux = a->aux; p.out = a->out; p.out2 = a->out2;
-  CAPE_REQUIRE(a->epilogue >= CAPE_EPI_LINEAR && a->epilogue <= CAPE_EPI_TANHGRAD, "unknown epilogue");
-  CAPE_REQUIRE(a->act >= CAPE_ACT_NONE && a->act <= CAPE_ACT_TANH, "unknown activation");
-  if (a->epilogue == CAPE_EPI_AFFINE) CAPE_REQUIRE(dual, "AFFINE epilogue needs a w2 term");
-  if (a->epilogue == CAPE_EPI_SLOPE || a->epilogue == CAPE_EPI_DUALMASK || a->epilogue == CAPE_EPI_TANHGRAD)
-    CAPE_REQUIRE(a->aux, "epilogue needs aux");
+  if (fill_epilogue(a, dual, &p.epi) != 0) return -1;
   p.wvec = wvec ? 1 : 0;
   p.ovec = (a->ncols % 4 == 0) && aligned16(a->out) && (!a->out2 || aligned16(a->out2)) && (!a->aux || aligned16(a->aux));
   const int BNsel = a->ncols <= 32 ? 32 : 64;
-  if (p.nslots > 0) {
-    const long long max_samples = (BM - 1) / a->rows_out + 2;
-    CAPE_REQUIRE(max_samples * p.nslots * BNsel <= BM * AS_STRIDE, "rows_out too small for the condition staging buffer");
-  }
+  CAPE_REQUIRE(max_tile_samples(BM, a->rows_out) * p.nslots * BNsel <= BM * AS_STRIDE,
+               "rows_out too small for the condition staging buffer");
   cudaStream_t st = (cudaStream_t)stream;
   if (a->plain_only) {
     const int rc = launch_gemm_tc(t, p, dual, st);
@@ -773,7 +695,7 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
   }
   // the fp32-pipe kernel with two accumulators (the affine block's forward) has no tanh epilogues: they would cost it
   // registers it spills already
-  CAPE_REQUIRE(!dual || (a->act != CAPE_ACT_TANH && a->epilogue != CAPE_EPI_TANHGRAD),
+  CAPE_REQUIRE(!dual || !needs_tanh(p.epi),
                "tanh / TANHGRAD epilogues with a w2 term need the tensor-core kernel (ncols % 32 == 0, wT / w2T given)");
   if (any_stash) {                                        // fp32-pipe path: the basis copies come from the resample kernel
     for (int i = 0; i < p.nterms; ++i) {
@@ -810,6 +732,19 @@ extern "C" int cape_cheb_fwd(cape_topology* t, const cape_conv_args* a, void* st
 
 static int dw_single(cape_topology* t, const cape_dw_args* a, void* stream);
 
+// sums the nsplit partial blocks [nsplit, F, ncols] of the workspace into dw (reduce_splits_kernel)
+static int reduce_splits(const cape_topology* t, int nsplit, int F, int ncols, float* dw, long long dw_stride,
+                         int accumulate, int Fper, long long term_stride, long long col_stride, cudaStream_t st) {
+  const long long total = (long long)F * ncols;
+  long long blocks = (total + 31) / 32;
+  if (blocks > 8LL * t->sm_count) blocks = 8LL * t->sm_count;
+  reduce_splits_kernel<<<(unsigned)blocks, 1024, 0, st>>>((const float*)t->workspace, nsplit, F, ncols, dw, dw_stride,
+                                                          accumulate, Fper, term_stride, col_stride);
+  CAPE_CHECK_CUDA(cudaGetLastError());
+  cape::count_launches(1);
+  return 0;
+}
+
 extern "C" int cape_cheb_dw(cape_topology* t, const cape_dw_args* a, void* stream) {
   CAPE_REQUIRE(t && a, "null handle/args");
   CAPE_REQUIRE(a->N > 0 && a->rows_out > 0 && a->ncols > 0 && a->F > 0, "empty problem");
@@ -827,17 +762,9 @@ extern "C" int cape_cheb_dw(cape_topology* t, const cape_dw_args* a, void* strea
   int ns = 1;
   int rc = launch_thin_dw(t, a, ops, a->nops, &ns, (cudaStream_t)stream);
   if (rc < 0) return rc;
-  if (rc == 1) {
-    const long long total = (long long)a->nops * a->F * a->ncols;
-    long long blocks = (total + 31) / 32;
-    if (blocks > 8LL * t->sm_count) blocks = 8LL * t->sm_count;
-    reduce_splits_kernel<<<(unsigned)blocks, 1024, 0, (cudaStream_t)stream>>>(
-        (const float*)t->workspace, ns, a->nops * a->F, a->ncols, a->dw, a->dw_stride, a->accumulate, a->F,
-        a->dw_term_stride, a->dw_col_stride > 0 ? a->dw_col_stride : 1);
-    CAPE_CHECK_CUDA(cudaGetLastError());
-    cape::count_launches(1);
-    return 0;
-  }
+  if (rc == 1)
+    return reduce_splits(t, ns, a->nops * a->F, a->ncols, a->dw, a->dw_stride, a->accumulate, a->F, a->dw_term_stride,
+                         a->dw_col_stride > 0 ? a->dw_col_stride : 1, (cudaStream_t)stream);
   CAPE_REQUIRE(a->dw_col_stride <= 1, "dw_col_stride is only implemented for thin inputs (F <= 4, ncols 32..256)");
   for (int j = 0; j < a->nops; ++j) {
     cape_dw_args b = *a;
@@ -860,16 +787,9 @@ static int dw_single(cape_topology* t, const cape_dw_args* a, void* stream) {
     else rc = launch_ellconv_dw_tc(t, a, p.op, &ns, (cudaStream_t)stream);        // tensor cores (wgmma)
     if (rc < 0) return rc;
     if (rc == 1) {
-      if (ns > 1 || always_reduce) {
-        const long long total = (long long)a->F * a->ncols;
-        long long blocks = (total + 31) / 32;
-        if (blocks > 8LL * t->sm_count) blocks = 8LL * t->sm_count;
-        reduce_splits_kernel<<<(unsigned)blocks, 1024, 0, (cudaStream_t)stream>>>((const float*)t->workspace, ns, a->F,
-                                                                                 a->ncols, a->dw, a->dw_stride,
-                                                                                 a->accumulate, a->F, 0, 1);
-        CAPE_CHECK_CUDA(cudaGetLastError());
-        cape::count_launches(1);
-      }
+      if (ns > 1 || always_reduce)
+        return reduce_splits(t, ns, a->F, a->ncols, a->dw, a->dw_stride, a->accumulate, a->F, 0, 1,
+                             (cudaStream_t)stream);
       return 0;
     }
   }
@@ -898,15 +818,8 @@ static int dw_single(cape_topology* t, const cape_dw_args* a, void* stream) {
   ellconv_dw_kernel<<<grid, NT, 0, st>>>(p);
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
-  if (nsplit > 1) {
-    const long long total = (long long)a->F * a->ncols;
-    long long blocks = (total + 31) / 32;
-    if (blocks > 8LL * t->sm_count) blocks = 8LL * t->sm_count;
-    reduce_splits_kernel<<<(unsigned)blocks, 1024, 0, st>>>((const float*)t->workspace, (int)nsplit, a->F, a->ncols, a->dw,
-                                                  a->dw_stride, a->accumulate, a->F, 0, 1);
-    CAPE_CHECK_CUDA(cudaGetLastError());
-  cape::count_launches(1);
-  }
+  if (nsplit > 1)
+    return reduce_splits(t, (int)nsplit, a->F, a->ncols, a->dw, a->dw_stride, a->accumulate, a->F, 0, 1, st);
   return 0;
 }
 

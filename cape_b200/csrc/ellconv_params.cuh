@@ -1,6 +1,7 @@
 // Parameter blocks shared by the SIMT (ellconv.cu) and wgmma (ellconv_tc.cu) fused-conv kernels.
 #pragma once
 #include "common.cuh"
+#include "epilogue.cuh"
 
 namespace cape {
 
@@ -33,34 +34,20 @@ struct ConvParams {
   int slot_term[MAX_SLOTS];
   int slot_acc[MAX_SLOTS];
   const float* slot_w[MAX_SLOTS];
+  int slot_ws[MAX_SLOTS];   // the term's w_stride or w2_stride
   const float* cond;
   int C;
-  int epilogue, act;
-  float alpha;
-  const float* bias;
-  int bias_per_row;
+  EpiParams epi;
   // terms[0, nterms) are contracted; terms[nterms, nterms + npass) are pass-through terms (cape_term with no weights:
   // acc0 += op . src[:, :, :ncols] in the epilogue).  A launcher that does not add them must decline a call with npass > 0.
   int npass;
-  const float* aux;
-  float* out;
-  float* out2;
   int wvec, ovec;
 };
 
 // One row of a pass-through term: sum_j op[r, j] * base[idx[r, j] * stride] (op.idx == nullptr: base[r * stride]), taps in
 // table order.  `base` points at the sample's source rows, offset by the column.
 __device__ __forceinline__ float pass_row(const OpView& op, int r, const float* base, size_t stride) {
-  if (op.idx == nullptr) return __ldg(base + (size_t)r * stride);
-  const int32_t* ip = op.idx + (size_t)r * op.width;
-  const float* wp = op.w + (size_t)r * op.width;
-  float v = 0.f;
-  for (int j = 0; j < op.width; ++j) {
-    const int id = __ldg(ip + j);
-    if (id < 0) break;
-    v = fmaf(__ldg(wp + j), __ldg(base + (size_t)id * stride), v);
-  }
-  return v;
+  return op.idx == nullptr ? __ldg(base + (size_t)r * stride) : ell_gather1(op, r, base, stride);
 }
 
 // the same for two adjacent columns (base 8-byte aligned, stride even)

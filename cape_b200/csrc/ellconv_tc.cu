@@ -129,8 +129,9 @@ __device__ __forceinline__ void ell_gather4_pairs(const OpView& op, const int (&
 // for the next launch of the handle.
 template <int BN, bool DUAL, bool PASS, bool TANH>
 __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_constant__ ConvParams p,
-                                                                  const __grid_constant__ WeightMaps maps, int nqs,
-                                                                  int ncol_tiles, int ntiles, unsigned* counter) {
+                                                                  const __grid_constant__ WeightMaps maps,
+                                                                  int max_samples, int ncol_tiles, int ntiles,
+                                                                  unsigned* counter) {
   using Cfg = ConvCfg<BN, DUAL>;
   constexpr int S = Cfg::STAGES;
   constexpr int NA = BN / 2;                  // accumulator registers per consumer thread
@@ -276,9 +277,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   // =========================== consumers ===========================
   setmaxnreg_inc<CONSUMER_REGS>();
   const int cw = wg - 2, ctid = tid - PRODUCER_THREADS;
-  const bool linear = p.epilogue == CAPE_EPI_LINEAR;
-  const bool use_aux =
-      p.epilogue == CAPE_EPI_SLOPE || p.epilogue == CAPE_EPI_DUALMASK || (TANH && p.epilogue == CAPE_EPI_TANHGRAD);
+  const EpiParams& e = p.epi;
+  const bool use_aux = epi_reads_aux(e.epilogue);
   uint32_t it = 0;                            // as the producers' count
   for (;;) {
     mbar_wait(&full[it % S], (it / S) & 1);   // the tile's first chunk carries its index
@@ -333,22 +333,11 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
     const int ct = tile % ncol_tiles;
     const long long row0 = (long long)(tile / ncol_tiles) * BM;
     const int col0 = ct * BN;
-    // condition broadcast vectors of this tile: qs[s][slot][c] = cond[n_first + s, :] . Wc_slot[:, col0 + c]
+    // condition broadcast vectors of this tile
     const int n_first = (int)(row0 / p.rows_out);
     if (p.nslots > 0) {
       named_bar_sync(1, CONSUMER_THREADS);    // the previous tile's epilogue has read qs
-      for (int o = ctid; o < nqs; o += CONSUMER_THREADS) {
-        const int c = o % BN, slot = (o / BN) % p.nslots, s = o / (BN * p.nslots);
-        float q = 0.f;
-        const int n = n_first + s;
-        if (col0 + c < p.ncols && n < p.N) {
-          const float* y = p.cond + (size_t)n * p.C;
-          const float* wc = p.slot_w[slot] + col0 + c;
-          const int ws = p.slot_acc[slot] ? p.terms[p.slot_term[slot]].w2_stride : p.terms[p.slot_term[slot]].w_stride;
-          for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * ws), q);
-        }
-        qs[o] = q;
-      }
+      stage_cond<16>(p, qs, n_first, min(max_samples, p.N - n_first), col0, BN, p.ncols, ctid, CONSUMER_THREADS);
       named_bar_sync(1, CONSUMER_THREADS);    // qs complete
     }
 
@@ -365,9 +354,8 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
       // condition slots, then pass-through terms, into the accumulators in place: each slot or term is a runtime loop
       // around the unrolled columns, so that the accumulators are only ever indexed by constants
       for (int slot = 0; slot < p.nslots; ++slot) {
-        const TermDev& tm = p.terms[p.slot_term[slot]];
-        const float coef = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
-        const float* q = qs + ((size_t)(n - n_first) * p.nslots + slot) * BN + frag_col(wt, 0);
+        const float coef = cond_coef(p.terms[p.slot_term[slot]].op, r);
+        const float* q = cond_vec(qs, n - n_first, slot, p.nslots, BN) + frag_col(wt, 0);
         if (p.slot_acc[slot] == 0) {
 #pragma unroll
           for (int g = 0; g < NA / 4; ++g) {
@@ -396,50 +384,23 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
           }
         }
       }
-      const float* bias_row = (linear && p.bias != nullptr) ? p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) : nullptr;
+      const float* bias_row = (e.epilogue == CAPE_EPI_LINEAR && e.bias != nullptr)
+                                  ? e.bias + (e.bias_per_row ? (size_t)r * p.ncols : 0) : nullptr;
 #pragma unroll
       for (int g = 0; g < NA / 4; ++g) {
         const int i = 4 * g + 2 * h;
         const int c = col0 + frag_col(wt, i);
         if (c >= p.ncols) continue;
-        float v0[2] = {acc0[i], acc0[i + 1]}, v1[2] = {0.f, 0.f};
+        float v0[2] = {acc0[i], acc0[i + 1]}, v1[2] = {0.f, 0.f}, b[2] = {0.f, 0.f}, ax[2] = {0.f, 0.f}, o1[2], o2[2];
         if (DUAL) { v1[0] = acc1[i]; v1[1] = acc1[i + 1]; }
-        float o1[2], o2[2];
-        bool write2 = false;
-        if (linear) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            float v = v0[e] + (bias_row != nullptr ? __ldg(bias_row + c + e) : 0.f);
-            if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
-            else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
-            else if (TANH && p.act == CAPE_ACT_TANH) v = tanhf(v);
-            o1[e] = v;
-          }
-        } else if (p.epilogue == CAPE_EPI_AFFINE) {
-          write2 = p.out2 != nullptr;
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float rg = fmaxf(v0[e], 0.f);
-            o1[e] = (DUAL ? v1[e] : 0.f) + rg;
-            o2[e] = rg;
-          }
-        } else {
-          const float2 ax = use_aux ? __ldg(reinterpret_cast<const float2*>(p.aux + orow + c)) : make_float2(0.f, 0.f);
-          const float a2[2] = {ax.x, ax.y};
-          if (p.epilogue == CAPE_EPI_SLOPE) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) o1[e] = v0[e] * (a2[e] > 0.f ? 1.f : p.alpha);
-          } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
-#pragma unroll
-            for (int e = 0; e < 2; ++e) o1[e] = v0[e] * (1.f - a2[e] * a2[e]);
-          } else {
-            write2 = p.out2 != nullptr;
-#pragma unroll
-            for (int e = 0; e < 2; ++e) { o1[e] = v0[e]; o2[e] = a2[e] > 0.f ? v0[e] : 0.f; }
-          }
+        if (bias_row != nullptr) { b[0] = __ldg(bias_row + c); b[1] = __ldg(bias_row + c + 1); }
+        if (use_aux) {
+          const float2 a2 = __ldg(reinterpret_cast<const float2*>(e.aux + orow + c));
+          ax[0] = a2.x; ax[1] = a2.y;
         }
-        *reinterpret_cast<float2*>(p.out + orow + c) = make_float2(o1[0], o1[1]);
-        if (write2) *reinterpret_cast<float2*>(p.out2 + orow + c) = make_float2(o2[0], o2[1]);
+        const bool write2 = apply_epilogue<TANH>(e, v0, v1, b, ax, o1, o2);
+        *reinterpret_cast<float2*>(e.out + orow + c) = make_float2(o1[0], o1[1]);
+        if (write2) *reinterpret_cast<float2*>(e.out2 + orow + c) = make_float2(o2[0], o2[1]);
       }
     };
     row_epilogue(std::integral_constant<int, 0>{});
@@ -493,13 +454,8 @@ int launch_conv_inst(const cape_topology* t, const ConvParams& p, cudaStream_t s
         encode_weight_map(&maps.w[i][1], tm.w2T, tm.F, tm.w2T_stride, p.ncols, BN) != 0)
       return -2;
   }
-  int nqs = 0;
-  if (p.nslots > 0) {
-    const long long rlast_max = BM - 1;
-    const int S = (int)(rlast_max / p.rows_out) + 2;
-    nqs = S * p.nslots * BN;
-  }
-  const int smem = 1024 + Cfg::RING + BAR_BYTES + nqs * 4;
+  const int max_samples = (int)max_tile_samples(BM, p.rows_out);
+  const int smem = 1024 + Cfg::RING + BAR_BYTES + max_samples * p.nslots * BN * 4;
   static bool configured = false;
   if (!configured) {
     CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL, PASS, TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -514,18 +470,18 @@ int launch_conv_inst(const cape_topology* t, const ConvParams& p, cudaStream_t s
     return -1;
   }
   const int grid = (int)std::min<long long>(ntiles, t->sm_count);
-  conv_wg_kernel<BN, DUAL, PASS, TANH><<<grid, CONV_THREADS, smem, st>>>(p, maps, nqs, ncol_tiles, (int)ntiles,
+  conv_wg_kernel<BN, DUAL, PASS, TANH><<<grid, CONV_THREADS, smem, st>>>(p, maps, max_samples, ncol_tiles, (int)ntiles,
                                                                    t->tile_counter);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;
 }
 
-// the tanh epilogues (b1tanh) in instantiations of their own: the precise tanhf, unrolled over a tile's columns, adds a
-// fifth to the kernel's code, which made the other activations' steps ~1 % slower as a run-time branch
+// the tanh epilogues in instantiations of their own: the precise tanhf, unrolled over a tile's columns, adds a fifth to
+// the kernel's code
 template <int BN, bool DUAL, bool PASS = false>
 int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
-  if (p.act == CAPE_ACT_TANH || p.epilogue == CAPE_EPI_TANHGRAD) return launch_conv_inst<BN, DUAL, PASS, true>(t, p, st);
+  if (needs_tanh(p.epi)) return launch_conv_inst<BN, DUAL, PASS, true>(t, p, st);
   return launch_conv_inst<BN, DUAL, PASS, false>(t, p, st);
 }
 
@@ -539,9 +495,7 @@ int pick_bn(int ncols, bool dual) {
 
 // false if the condition vectors of a tile would not fit the staging buffer
 bool qs_fits(const ConvParams& p, int bn) {
-  if (p.nslots == 0) return true;
-  const long long max_samples = (BM - 1) / p.rows_out + 2;
-  return max_samples * p.nslots * bn <= QS_MAX_FLOATS;
+  return max_tile_samples(BM, p.rows_out) * p.nslots * bn <= QS_MAX_FLOATS;
 }
 
 }  // namespace
@@ -582,7 +536,7 @@ int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cu
 // all-plain-operand calls: 1 = launched, 0 = not eligible (the caller falls through to the gather kernels)
 int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
   if (!tensor_cores_enabled() || g_tuning[8] == 1) return 0;
-  if (dual || p.epilogue == CAPE_EPI_AFFINE || p.npass > 0) return 0;
+  if (dual || p.epi.epilogue == CAPE_EPI_AFFINE || p.npass > 0) return 0;
   if (p.ncols % 16 != 0 || p.ncols < 32 || !p.ovec) return 0;
   if (p.total_rows >= (1LL << 31)) return 0;
   long long kred = 0;

@@ -3,6 +3,7 @@
 // These are weight-bandwidth bound (2 x 55168x64 + 128x55168 fp32 = 56.7 MB read once per pass at batch 64),
 // so the contraction stays on the fp32 pipe; split-K over the 55168-long reduction fills the SMs.
 #include "common.cuh"
+#include "epilogue.cuh"
 #include "ellconv_params.cuh"
 
 namespace cape {
@@ -20,12 +21,6 @@ struct GemmParams {
   int nsplit, k_per_split;
   float* ws;
 };
-
-__device__ __forceinline__ float apply_act(float v, int act, float leaky) {
-  if (act == CAPE_ACT_LEAKY) return v > 0.f ? v : leaky * v;
-  if (act == CAPE_ACT_RELU) return fmaxf(v, 0.f);
-  return v;
-}
 
 __device__ __forceinline__ void gemm_load(const GemmParams& p, int m0, int n0, int k0, int kend, int tid,
                                           float (&ra)[4], float (&rb)[4]) {
@@ -132,7 +127,7 @@ __device__ __forceinline__ void gemm_tile(const GemmParams& p, int m0, int n0, i
       } else {
         float v = p.alpha * acc[i][j];
         if (p.bias) v += __ldg(p.bias + n);
-        v = apply_act(v, p.act, p.leaky);
+        v = activate<false>(v, p.act, p.leaky);
         float* o = p.c + (size_t)m * p.c_rs + n;
         if (p.beta != 0.f) v += p.beta * (*o);
         *o = v;
@@ -253,7 +248,7 @@ __global__ void __launch_bounds__(256, 3) gemm_vec_kernel(const __grid_constant_
       } else {
         float v = p.alpha * acc[i][j];
         if (p.bias) v += __ldg(p.bias + n);
-        v = apply_act(v, p.act, p.leaky);
+        v = activate<false>(v, p.act, p.leaky);
         float* o = p.c + (size_t)m * p.c_rs + n;
         if (p.beta != 0.f) v += p.beta * (*o);
         *o = v;
@@ -298,7 +293,7 @@ __global__ void __launch_bounds__(GR_EL * GR_ZL) gemm_reduce_kernel(const __grid
       const int m = (int)(e / p.N), n = (int)(e % p.N);
       float v = p.alpha * s;
       if (p.bias) v += __ldg(p.bias + n);
-      v = apply_act(v, p.act, p.leaky);
+      v = activate<false>(v, p.act, p.leaky);
       float* o = p.c + (size_t)m * p.c_rs + n;
       if (p.beta != 0.f) v += p.beta * (*o);
       *o = v;

@@ -54,7 +54,7 @@ __device__ __forceinline__ void thin_gather(const OpView& op, int r, const float
   }
 }
 
-// TANH: the tanh epilogues (b1tanh), compiled only into instantiations of their own (as in conv_wg_kernel)
+// TANH: the tanh epilogues (needs_tanh)
 template <bool TANH>
 __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ ConvParams p, int KF, int vec4) {
   __shared__ float Bs[TH_ROWS][TH_MAXKF + 1];
@@ -102,18 +102,10 @@ __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ C
     int n_last = n_first;
     for (int i = TH_ROWS - 1; i > 0; --i)
       if (s_n[i] >= 0) { n_last = s_n[i]; break; }
-    const int S = n_last - n_first + 1;
-    for (int o = tid; o < S * p.nslots * ncols; o += 256) {
-      const int c = o % ncols, slot = (o / ncols) % p.nslots, s = o / (ncols * p.nslots);
-      const float* y = p.cond + (size_t)(n_first + s) * p.C;
-      const float* wc = p.slot_w[slot] + c;
-      const int ws = p.terms[p.slot_term[slot]].w_stride;
-      float q = 0.f;
-      for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(wc + (size_t)j * ws), q);
-      qs[o] = q;
-    }
+    stage_cond<16>(p, qs, n_first, n_last - n_first + 1, 0, ncols, ncols, tid, 256);
   }
   __syncthreads();
+  const EpiParams& e = p.epi;
 
   // ---- phase 2: outputs, coalesced along the columns -- four columns per thread when everything is 16-byte aligned
   if (vec4) {
@@ -125,43 +117,22 @@ __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ C
       const int r = s_r[row];
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
       for (int q = 0; q < KF; ++q) fma4(acc, Bs[row][q], *reinterpret_cast<const float4*>(&Ws[q * ncols + c]));
-      for (int slot = 0; slot < p.nslots; ++slot) {
-        const TermDev& tm = p.terms[p.slot_term[slot]];
-        const float coef = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
-        fma4(acc, coef, *reinterpret_cast<const float4*>(&qs[((n - n_first) * p.nslots + slot) * ncols + c]));
-      }
+      for (int slot = 0; slot < p.nslots; ++slot)
+        fma4(acc, cond_coef(p.terms[p.slot_term[slot]].op, r),
+             *reinterpret_cast<const float4*>(cond_vec(qs, n - n_first, slot, p.nslots, ncols) + c));
       const size_t oi = (size_t)(row0 + row) * ncols + c;
-      if (p.epilogue == CAPE_EPI_LINEAR) {
-        if (p.bias != nullptr) {
-          const float4 b = ldg4(p.bias + (p.bias_per_row ? (size_t)r * ncols : 0) + c);
-          acc.x += b.x; acc.y += b.y; acc.z += b.z; acc.w += b.w;
-        }
-        if (p.act == CAPE_ACT_LEAKY) {
-          acc.x = acc.x > 0.f ? acc.x : p.alpha * acc.x; acc.y = acc.y > 0.f ? acc.y : p.alpha * acc.y;
-          acc.z = acc.z > 0.f ? acc.z : p.alpha * acc.z; acc.w = acc.w > 0.f ? acc.w : p.alpha * acc.w;
-        } else if (p.act == CAPE_ACT_RELU) {
-          acc.x = fmaxf(acc.x, 0.f); acc.y = fmaxf(acc.y, 0.f); acc.z = fmaxf(acc.z, 0.f); acc.w = fmaxf(acc.w, 0.f);
-        } else if (TANH && p.act == CAPE_ACT_TANH) {
-          acc.x = tanhf(acc.x); acc.y = tanhf(acc.y); acc.z = tanhf(acc.z); acc.w = tanhf(acc.w);
-        }
-        *reinterpret_cast<float4*>(p.out + oi) = acc;
-      } else {
-        const float4 a = ldg4(p.aux + oi);
-        if (p.epilogue == CAPE_EPI_SLOPE) {
-          *reinterpret_cast<float4*>(p.out + oi) =
-              make_float4(acc.x * (a.x > 0.f ? 1.f : p.alpha), acc.y * (a.y > 0.f ? 1.f : p.alpha),
-                          acc.z * (a.z > 0.f ? 1.f : p.alpha), acc.w * (a.w > 0.f ? 1.f : p.alpha));
-        } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
-          *reinterpret_cast<float4*>(p.out + oi) =
-              make_float4(acc.x * (1.f - a.x * a.x), acc.y * (1.f - a.y * a.y), acc.z * (1.f - a.z * a.z),
-                          acc.w * (1.f - a.w * a.w));
-        } else {  // DUALMASK
-          *reinterpret_cast<float4*>(p.out + oi) = acc;
-          if (p.out2 != nullptr)
-            *reinterpret_cast<float4*>(p.out2 + oi) = make_float4(a.x > 0.f ? acc.x : 0.f, a.y > 0.f ? acc.y : 0.f,
-                                                                  a.z > 0.f ? acc.z : 0.f, a.w > 0.f ? acc.w : 0.f);
-        }
+      float v0[4] = {acc.x, acc.y, acc.z, acc.w}, zero[4] = {0.f, 0.f, 0.f, 0.f}, b[4] = {0.f, 0.f, 0.f, 0.f};
+      float ax[4] = {0.f, 0.f, 0.f, 0.f}, o1[4], o2[4];
+      if (e.epilogue == CAPE_EPI_LINEAR && e.bias != nullptr) {
+        const float4 b4 = ldg4(e.bias + (e.bias_per_row ? (size_t)r * ncols : 0) + c);
+        b[0] = b4.x; b[1] = b4.y; b[2] = b4.z; b[3] = b4.w;
+      } else if (epi_reads_aux(e.epilogue)) {
+        const float4 a4 = ldg4(e.aux + oi);
+        ax[0] = a4.x; ax[1] = a4.y; ax[2] = a4.z; ax[3] = a4.w;
       }
+      const bool write2 = apply_epilogue<TANH>(e, v0, zero, b, ax, o1, o2);
+      *reinterpret_cast<float4*>(e.out + oi) = make_float4(o1[0], o1[1], o1[2], o1[3]);
+      if (write2) *reinterpret_cast<float4*>(e.out2 + oi) = make_float4(o2[0], o2[1], o2[2], o2[3]);
     }
     return;
   }
@@ -172,27 +143,15 @@ __global__ void __launch_bounds__(256) thin_fwd_kernel(const __grid_constant__ C
     const int r = s_r[row];
     float acc = 0.f;
     for (int q = 0; q < KF; ++q) acc = fmaf(Bs[row][q], Ws[q * ncols + c], acc);
-    for (int slot = 0; slot < p.nslots; ++slot) {
-      const TermDev& tm = p.terms[p.slot_term[slot]];
-      const float coef = tm.op.rowsum ? __ldg(tm.op.rowsum + r) : 1.f;
-      acc = fmaf(coef, qs[((n - n_first) * p.nslots + slot) * ncols + c], acc);
-    }
+    for (int slot = 0; slot < p.nslots; ++slot)
+      acc = fmaf(cond_coef(p.terms[p.slot_term[slot]].op, r), cond_vec(qs, n - n_first, slot, p.nslots, ncols)[c], acc);
     const size_t oi = (size_t)(row0 + row) * ncols + c;
-    if (p.epilogue == CAPE_EPI_LINEAR) {
-      if (p.bias != nullptr) acc += __ldg(p.bias + (p.bias_per_row ? (size_t)r * ncols : 0) + c);
-      if (p.act == CAPE_ACT_LEAKY) acc = acc > 0.f ? acc : p.alpha * acc;
-      else if (p.act == CAPE_ACT_RELU) acc = fmaxf(acc, 0.f);
-      else if (TANH && p.act == CAPE_ACT_TANH) acc = tanhf(acc);
-      p.out[oi] = acc;
-    } else if (p.epilogue == CAPE_EPI_SLOPE) {
-      p.out[oi] = acc * (__ldg(p.aux + oi) > 0.f ? 1.f : p.alpha);
-    } else if (TANH && p.epilogue == CAPE_EPI_TANHGRAD) {
-      const float a = __ldg(p.aux + oi);
-      p.out[oi] = acc * (1.f - a * a);
-    } else {  // DUALMASK
-      p.out[oi] = acc;
-      if (p.out2 != nullptr) p.out2[oi] = __ldg(p.aux + oi) > 0.f ? acc : 0.f;
-    }
+    float v0[1] = {acc}, zero[1] = {0.f}, b[1] = {0.f}, ax[1] = {0.f}, o1[1], o2[1];
+    if (e.epilogue == CAPE_EPI_LINEAR && e.bias != nullptr)
+      b[0] = __ldg(e.bias + (e.bias_per_row ? (size_t)r * ncols : 0) + c);
+    else if (epi_reads_aux(e.epilogue)) ax[0] = __ldg(e.aux + oi);
+    if (apply_epilogue<TANH>(e, v0, zero, b, ax, o1, o2)) e.out2[oi] = o2[0];
+    e.out[oi] = o1[0];
   }
 }
 
@@ -339,31 +298,19 @@ struct ThinOutParams {
   const float* slot_w[TO_MAXT];
   int slot_ws[TO_MAXT];
   const float* cond;
-  const float* bias;
-  int bias_per_row, act;
-  float alpha;
-  float* out;
+  EpiParams epi;       // LINEAR
 };
 
 constexpr int TO_MAXS = 8;        // samples a 256-row block may touch
 
 __global__ void __launch_bounds__(256) thinout_combine_kernel(const __grid_constant__ ThinOutParams p) {
-  __shared__ float qs[TO_MAXS][TO_MAXT][4];
+  __shared__ float qs[TO_MAXS * TO_MAXT * 4];
   const long long R0 = (long long)blockIdx.x * 256;
   const int n_first = (int)(R0 / p.rows_out);
   if (p.nslots > 0) {
-    // condition vectors of the samples in this block: q[s][slot][c] = cond[n_first+s,:] @ Wc_slot[:, c]
+    // condition vectors of the samples in this block
     const long long rlast = min(p.total_rows, R0 + 256) - 1;
-    const int S = (int)(rlast / p.rows_out) - n_first + 1;
-    for (int o = threadIdx.x; o < S * p.nslots * 4; o += 256) {
-      const int c = o & 3, slot = (o >> 2) % p.nslots, s = (o >> 2) / p.nslots;
-      float q = 0.f;
-      if (c < p.ncols) {
-        const float* y = p.cond + (size_t)(n_first + s) * p.C;
-        for (int j = 0; j < p.C; ++j) q = fmaf(__ldg(y + j), __ldg(p.slot_w[slot] + (size_t)j * p.slot_ws[slot] + c), q);
-      }
-      qs[s][slot][c] = q;
-    }
+    stage_cond<4>(p, qs, n_first, (int)(rlast / p.rows_out) - n_first + 1, 0, 4, p.ncols, threadIdx.x, 256);
     __syncthreads();
   }
   const long long R = R0 + threadIdx.x;
@@ -394,18 +341,16 @@ __global__ void __launch_bounds__(256) thinout_combine_kernel(const __grid_const
     }
   }
   for (int s = 0; s < p.nslots; ++s) {
-    const OpView& op = p.op[p.slot_term[s]];
-    const float coef = op.rowsum ? __ldg(op.rowsum + r) : 1.f;
+    const float coef = cond_coef(p.op[p.slot_term[s]], r);
+    const float* q = cond_vec(qs, n - n_first, s, p.nslots, 4);
 #pragma unroll
-    for (int c = 0; c < 4; ++c) acc[c] = fmaf(coef, qs[n - n_first][s][c], acc[c]);
+    for (int c = 0; c < 4; ++c) acc[c] = fmaf(coef, q[c], acc[c]);
   }
+  const EpiParams& e = p.epi;
   for (int c = 0; c < p.ncols; ++c) {
     float v = acc[c];
-    if (p.bias != nullptr) v += __ldg(p.bias + (p.bias_per_row ? (size_t)r * p.ncols : 0) + c);
-    if (p.act == CAPE_ACT_LEAKY) v = v > 0.f ? v : p.alpha * v;
-    else if (p.act == CAPE_ACT_RELU) v = fmaxf(v, 0.f);
-    else if (p.act == CAPE_ACT_TANH) v = tanhf(v);
-    p.out[(size_t)R * p.ncols + c] = v;
+    if (e.bias != nullptr) v += __ldg(e.bias + (e.bias_per_row ? (size_t)r * p.ncols : 0) + c);
+    e.out[(size_t)R * p.ncols + c] = activate<true>(v, e.act, e.alpha);
   }
 }
 
@@ -414,7 +359,7 @@ __global__ void __launch_bounds__(256) thinout_combine_kernel(const __grid_const
 // returns 1 if launched, 0 if not eligible
 int launch_thin_fwd(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
   (void)t;
-  if (dual || p.epilogue == CAPE_EPI_AFFINE || p.npass > 0) return 0;   // pass-through terms: ellconv kernels
+  if (dual || p.epi.epilogue == CAPE_EPI_AFFINE || p.npass > 0) return 0;   // pass-through terms: ellconv kernels
   if (p.ncols > TH_MAXCOLS || p.ncols < 16) return 0;
   int KF = 0;
   for (int i = 0; i < p.nterms; ++i) {
@@ -422,15 +367,12 @@ int launch_thin_fwd(const cape_topology* t, const ConvParams& p, bool dual, cuda
     KF += p.terms[i].F;
   }
   if (KF > TH_MAXKF) return 0;
-  if (p.nslots > 0) {
-    const long long max_samples = (TH_ROWS - 1) / p.rows_out + 2;
-    if (max_samples * p.nslots * p.ncols > TH_QS) return 0;
-    for (int s = 0; s < p.nslots; ++s)
-      if (p.slot_acc[s] != 0) return 0;
-  }
+  if (max_tile_samples(TH_ROWS, p.rows_out) * p.nslots * p.ncols > TH_QS) return 0;
+  for (int s = 0; s < p.nslots; ++s)
+    if (p.slot_acc[s] != 0) return 0;
   const unsigned grid = (unsigned)((p.total_rows + TH_ROWS - 1) / TH_ROWS);
-  const int vec4 = (p.ncols % 4 == 0) && p.ovec && (p.bias == nullptr || aligned16(p.bias));
-  if (p.act == CAPE_ACT_TANH || p.epilogue == CAPE_EPI_TANHGRAD) thin_fwd_kernel<true><<<grid, 256, 0, st>>>(p, KF, vec4);
+  const int vec4 = (p.ncols % 4 == 0) && p.ovec && (p.epi.bias == nullptr || aligned16(p.epi.bias));
+  if (needs_tanh(p.epi)) thin_fwd_kernel<true><<<grid, 256, 0, st>>>(p, KF, vec4);
   else thin_fwd_kernel<false><<<grid, 256, 0, st>>>(p, KF, vec4);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
@@ -474,7 +416,7 @@ int launch_thin_dw(const cape_topology* t, const cape_dw_args* a, const OpView* 
 
 // thin-output conv: 1 = launched (z lives in the topology workspace), 0 = not eligible
 int launch_thinout_fwd(const cape_topology* t, const ConvParams& p, bool dual, cudaStream_t st) {
-  if (dual || p.epilogue != CAPE_EPI_LINEAR || p.ncols > 4 || p.nterms > TO_MAXT || p.npass > 0 || g_tuning[7] == 1)
+  if (dual || p.epi.epilogue != CAPE_EPI_LINEAR || p.ncols > 4 || p.nterms > TO_MAXT || p.npass > 0 || g_tuning[7] == 1)
     return 0;
   const TermDev& t0 = p.terms[0];
   if (!t0.vec || t0.F < 32 || t0.F % 4 != 0 || t0.F > 512) return 0;
@@ -484,7 +426,7 @@ int launch_thinout_fwd(const cape_topology* t, const ConvParams& p, bool dual, c
         tm.stash != nullptr)
       return 0;
   }
-  if (p.nslots > TO_MAXT || (p.nslots > 0 && 255 / p.rows_out + 2 > TO_MAXS)) return 0;
+  if (p.nslots > TO_MAXT || (p.nslots > 0 && max_tile_samples(256, p.rows_out) > TO_MAXS)) return 0;
   for (int s = 0; s < p.nslots; ++s)
     if (p.slot_acc[s] != 0) return 0;
   const long long nsrc = (long long)p.N * t0.src_rows;
@@ -509,9 +451,9 @@ int launch_thinout_fwd(const cape_topology* t, const ConvParams& p, bool dual, c
   for (int i = 0; i < p.nterms; ++i) q.op[i] = p.terms[i].op;
   q.z = z; q.nslots = p.nslots; q.C = p.C; q.cond = p.cond;
   for (int s = 0; s < p.nslots; ++s) {
-    q.slot_term[s] = p.slot_term[s]; q.slot_w[s] = p.slot_w[s]; q.slot_ws[s] = p.terms[p.slot_term[s]].w_stride;
+    q.slot_term[s] = p.slot_term[s]; q.slot_w[s] = p.slot_w[s]; q.slot_ws[s] = p.slot_ws[s];
   }
-  q.bias = p.bias; q.bias_per_row = p.bias_per_row; q.act = p.act; q.alpha = p.alpha; q.out = p.out;
+  q.epi = p.epi;
   thinout_combine_kernel<<<(unsigned)((p.total_rows + 255) / 256), 256, 0, st>>>(q);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(2);

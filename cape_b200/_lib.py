@@ -84,6 +84,9 @@ SIGNATURES = {
     "cape_gemm": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
                             C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_float, C.c_float,
                             C.c_float, C.c_void_p]),
+    "cape_gemm_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p,
+                               C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_float, C.c_float,
+                               C.c_float, C.c_int, C.c_float, C.c_void_p, C.c_int64, C.c_void_p]),
     "cape_resample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                 C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
     "cape_cheb_weight_transpose": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),

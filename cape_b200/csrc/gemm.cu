@@ -20,7 +20,21 @@ struct GemmParams {
   float leaky, alpha, beta;
   int nsplit, k_per_split;
   float* ws;
+  // cape_gemm_ex: the data-gradient epilogue applied last (instantiations with BWD = true only)
+  EpiParams epi;
+  long long aux_rs;
 };
+
+// The finished output value v of element (m, n) through the data-gradient epilogue (SLOPE / TANHGRAD of epilogue.cuh,
+// given aux(m, n)); BWD = false compiles it out.
+template <bool BWD>
+__device__ __forceinline__ float gemm_bwd_epi(const GemmParams& p, float v, int m, int n) {
+  if (!BWD) return v;
+  const float v0[1] = {v}, zero[1] = {0.f}, aux[1] = {__ldg(p.epi.aux + (size_t)m * p.aux_rs + n)};
+  float o1[1], o2[1];
+  apply_epilogue<true, 1>(p.epi, v0, zero, zero, aux, o1, o2);
+  return o1[0];
+}
 
 __device__ __forceinline__ void gemm_load(const GemmParams& p, int m0, int n0, int k0, int kend, int tid,
                                           float (&ra)[4], float (&rb)[4]) {
@@ -80,6 +94,7 @@ __device__ __forceinline__ void gemm_store(const GemmParams& p, int tid, const f
 
 // One 64 x 64 output tile over the reduction range [kbeg, kend).  mode 0: epilogue store (alpha, bias, act, beta),
 // 1: raw partial sums to the split-K workspace slice `z`, 2: alpha * acc added atomically to c (batched accumulations).
+template <bool BWD = false>
 __device__ __forceinline__ void gemm_tile(const GemmParams& p, int m0, int n0, int kbeg, int kend, int z, int mode,
                                           float* As, float* Bs) {
   const int tid = threadIdx.x;
@@ -130,17 +145,18 @@ __device__ __forceinline__ void gemm_tile(const GemmParams& p, int m0, int n0, i
         v = activate<false>(v, p.act, p.leaky);
         float* o = p.c + (size_t)m * p.c_rs + n;
         if (p.beta != 0.f) v += p.beta * (*o);
-        *o = v;
+        *o = gemm_bwd_epi<BWD>(p, v, m, n);
       }
     }
   }
 }
 
+template <bool BWD>
 __global__ void __launch_bounds__(256, 2) gemm_kernel(const __grid_constant__ GemmParams p) {
   __shared__ __align__(16) float As[G_BK * G_STRIDE];
   __shared__ __align__(16) float Bs[G_BK * G_STRIDE];
   const int kbeg = blockIdx.z * p.k_per_split;
-  gemm_tile(p, blockIdx.y * G_BM, blockIdx.x * G_BN, kbeg, min(p.K, kbeg + p.k_per_split), blockIdx.z,
+  gemm_tile<BWD>(p, blockIdx.y * G_BM, blockIdx.x * G_BN, kbeg, min(p.K, kbeg + p.k_per_split), blockIdx.z,
             p.nsplit > 1 ? 1 : 0, As, Bs);
 }
 
@@ -201,7 +217,7 @@ __device__ __forceinline__ void gv_store(int tid, const float4 (&ra)[2], const f
   }
 }
 
-template <bool AK, bool BN>
+template <bool AK, bool BN, bool BWD>
 __global__ void __launch_bounds__(256, 3) gemm_vec_kernel(const __grid_constant__ GemmParams p) {
   __shared__ __align__(16) float As[GV_BK * G_STRIDE];
   __shared__ __align__(16) float Bs[GV_BK * G_STRIDE];
@@ -251,7 +267,7 @@ __global__ void __launch_bounds__(256, 3) gemm_vec_kernel(const __grid_constant_
         v = activate<false>(v, p.act, p.leaky);
         float* o = p.c + (size_t)m * p.c_rs + n;
         if (p.beta != 0.f) v += p.beta * (*o);
-        *o = v;
+        *o = gemm_bwd_epi<BWD>(p, v, m, n);
       }
     }
   }
@@ -273,6 +289,7 @@ __global__ void __launch_bounds__(256, 2) gemm_batch_kernel(const GemmParams* __
 // 32 split lanes per CTA, every lane adds its partials in index order, the lanes are added in index order through
 // shared memory -- a fixed summation order (deterministic, bit-identical on every replica).
 constexpr int GR_EL = 32, GR_ZL = 32;
+template <bool BWD>
 __global__ void __launch_bounds__(GR_EL * GR_ZL) gemm_reduce_kernel(const __grid_constant__ GemmParams p) {
   __shared__ float red[GR_ZL][GR_EL + 1];
   const long long total = (long long)p.M * p.N;
@@ -296,7 +313,7 @@ __global__ void __launch_bounds__(GR_EL * GR_ZL) gemm_reduce_kernel(const __grid
       v = activate<false>(v, p.act, p.leaky);
       float* o = p.c + (size_t)m * p.c_rs + n;
       if (p.beta != 0.f) v += p.beta * (*o);
-      *o = v;
+      *o = gemm_bwd_epi<BWD>(p, v, m, n);
     }
     __syncthreads();
   }
@@ -306,21 +323,19 @@ __global__ void __launch_bounds__(GR_EL * GR_ZL) gemm_reduce_kernel(const __grid
 
 using namespace cape;
 
-extern "C" int cape_gemm(cape_topology* t, int M, int N, int K, const float* a, int64_t a_rs, int64_t a_cs,
-                         const float* b, int64_t b_rs, int64_t b_cs, float* c, int64_t c_rs, const float* bias,
-                         int act, float leaky_alpha, float alpha, float beta, void* stream) {
-  CAPE_REQUIRE(t && a && b && c, "null pointer");
+// cape_gemm / cape_gemm_ex: one launch (plus the split-K reduction), BWD = the data-gradient epilogue's instantiations
+static int gemm_launch(cape_topology* t, GemmParams& p, bool bwd, void* stream) {
+  const int M = p.M, N = p.N, K = p.K;
+  CAPE_REQUIRE(t && p.a && p.b && p.c, "null pointer");
   CAPE_REQUIRE(M > 0 && N > 0 && K > 0, "empty problem");
-  CAPE_REQUIRE(a_cs == 1 || a_rs == 1, "A needs a unit stride");
-  CAPE_REQUIRE(b_cs == 1 || b_rs == 1, "B needs a unit stride");
+  CAPE_REQUIRE(p.a_cs == 1 || p.a_rs == 1, "A needs a unit stride");
+  CAPE_REQUIRE(p.b_cs == 1 || p.b_rs == 1, "B needs a unit stride");
   // the dense layers of the reference are fixed to leaky ReLU or none (models.py:496-510,557-582): no tanh here
-  CAPE_REQUIRE(act == CAPE_ACT_NONE || act == CAPE_ACT_LEAKY || act == CAPE_ACT_RELU,
+  CAPE_REQUIRE(p.act == CAPE_ACT_NONE || p.act == CAPE_ACT_LEAKY || p.act == CAPE_ACT_RELU,
                "cape_gemm implements ACT_NONE, ACT_LEAKY and ACT_RELU");
-  GemmParams p{};
-  p.M = M; p.N = N; p.K = K;
-  p.a = a; p.a_rs = a_rs; p.a_cs = a_cs;
-  p.b = b; p.b_rs = b_rs; p.b_cs = b_cs;
-  p.c = c; p.c_rs = c_rs; p.bias = bias; p.act = act; p.leaky = leaky_alpha; p.alpha = alpha; p.beta = beta;
+  const float* a = p.a;
+  const float* b = p.b;
+  const int64_t a_rs = p.a_rs, a_cs = p.a_cs, b_rs = p.b_rs, b_cs = p.b_cs;
   const int mt = (M + G_BM - 1) / G_BM, nt = (N + G_BN - 1) / G_BN;
   const long long tiles = (long long)mt * nt;
   // the vectorised kernel: worth it from ~1 MB of operands; every 16-byte vector aligned and inside its axis
@@ -348,22 +363,65 @@ extern "C" int cape_gemm(cape_topology* t, int M, int N, int K, const float* a, 
   CAPE_REQUIRE(mt <= 65535 && nsplit <= 65535, "grid too large");
   dim3 grid(nt, mt, (unsigned)nsplit);
   cudaStream_t st = (cudaStream_t)stream;
-  if (!vec) gemm_kernel<<<grid, 256, 0, st>>>(p);
-  else if (a_k && b_n) gemm_vec_kernel<true, true><<<grid, 256, 0, st>>>(p);
-  else if (a_k) gemm_vec_kernel<true, false><<<grid, 256, 0, st>>>(p);
-  else if (b_n) gemm_vec_kernel<false, true><<<grid, 256, 0, st>>>(p);
-  else gemm_vec_kernel<false, false><<<grid, 256, 0, st>>>(p);
+  if (bwd) {
+    if (!vec) gemm_kernel<true><<<grid, 256, 0, st>>>(p);
+    else if (a_k && b_n) gemm_vec_kernel<true, true, true><<<grid, 256, 0, st>>>(p);
+    else if (a_k) gemm_vec_kernel<true, false, true><<<grid, 256, 0, st>>>(p);
+    else if (b_n) gemm_vec_kernel<false, true, true><<<grid, 256, 0, st>>>(p);
+    else gemm_vec_kernel<false, false, true><<<grid, 256, 0, st>>>(p);
+  } else {
+    if (!vec) gemm_kernel<false><<<grid, 256, 0, st>>>(p);
+    else if (a_k && b_n) gemm_vec_kernel<true, true, false><<<grid, 256, 0, st>>>(p);
+    else if (a_k) gemm_vec_kernel<true, false, false><<<grid, 256, 0, st>>>(p);
+    else if (b_n) gemm_vec_kernel<false, true, false><<<grid, 256, 0, st>>>(p);
+    else gemm_vec_kernel<false, false, false><<<grid, 256, 0, st>>>(p);
+  }
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   if (nsplit > 1) {
     const long long total = (long long)M * N;
     long long blocks = (total + GR_EL - 1) / GR_EL;
     if (blocks > 8LL * t->sm_count) blocks = 8LL * t->sm_count;
-    gemm_reduce_kernel<<<(unsigned)blocks, GR_EL * GR_ZL, 0, st>>>(p);
+    if (bwd) gemm_reduce_kernel<true><<<(unsigned)blocks, GR_EL * GR_ZL, 0, st>>>(p);
+    else gemm_reduce_kernel<false><<<(unsigned)blocks, GR_EL * GR_ZL, 0, st>>>(p);
     CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   }
   return 0;
+}
+
+static GemmParams gemm_params(int M, int N, int K, const float* a, int64_t a_rs, int64_t a_cs, const float* b,
+                              int64_t b_rs, int64_t b_cs, float* c, int64_t c_rs, const float* bias, int act,
+                              float leaky_alpha, float alpha, float beta) {
+  GemmParams p{};
+  p.M = M; p.N = N; p.K = K;
+  p.a = a; p.a_rs = a_rs; p.a_cs = a_cs;
+  p.b = b; p.b_rs = b_rs; p.b_cs = b_cs;
+  p.c = c; p.c_rs = c_rs; p.bias = bias; p.act = act; p.leaky = leaky_alpha; p.alpha = alpha; p.beta = beta;
+  return p;
+}
+
+extern "C" int cape_gemm(cape_topology* t, int M, int N, int K, const float* a, int64_t a_rs, int64_t a_cs,
+                         const float* b, int64_t b_rs, int64_t b_cs, float* c, int64_t c_rs, const float* bias,
+                         int act, float leaky_alpha, float alpha, float beta, void* stream) {
+  GemmParams p = gemm_params(M, N, K, a, a_rs, a_cs, b, b_rs, b_cs, c, c_rs, bias, act, leaky_alpha, alpha, beta);
+  return gemm_launch(t, p, false, stream);
+}
+
+extern "C" int cape_gemm_ex(cape_topology* t, int M, int N, int K, const float* a, int64_t a_rs, int64_t a_cs,
+                            const float* b, int64_t b_rs, int64_t b_cs, float* c, int64_t c_rs, const float* bias,
+                            int act, float leaky_alpha, float alpha, float beta, int epilogue, float epi_alpha,
+                            const float* aux, int64_t aux_rs, void* stream) {
+  CAPE_REQUIRE(epilogue == CAPE_EPI_LINEAR || epilogue == CAPE_EPI_SLOPE || epilogue == CAPE_EPI_TANHGRAD,
+               "cape_gemm_ex implements the LINEAR, SLOPE and TANHGRAD epilogues");
+  CAPE_REQUIRE(epilogue == CAPE_EPI_LINEAR || aux, "epilogue needs aux");
+  GemmParams p = gemm_params(M, N, K, a, a_rs, a_cs, b, b_rs, b_cs, c, c_rs, bias, act, leaky_alpha, alpha, beta);
+  const bool bwd = epilogue != CAPE_EPI_LINEAR;
+  if (bwd) {
+    p.epi = EpiParams{epilogue, CAPE_ACT_NONE, epi_alpha, nullptr, 0, aux, c, nullptr};
+    p.aux_rs = aux_rs;
+  }
+  return gemm_launch(t, p, bwd, stream);
 }
 
 extern "C" int cape_gemm_batch(const cape_gemm_item* items_host, int n, void* table_device, int blocks_per_item,

@@ -158,12 +158,21 @@ class ConvSite:
 # ---------------------------------------------------------------------------------------------------
 # kernel-call helpers
 # ---------------------------------------------------------------------------------------------------
-def gemm(tp, A, B, Cout, bias=None, act=ACT_NONE, alpha=1.0, beta=0.0, tag=None):
-    """Cout = act(alpha * A @ B + bias) + beta * Cout for 2-D (possibly transposed) views."""
+def gemm(tp, A, B, Cout, bias=None, act=ACT_NONE, alpha=1.0, beta=0.0, tag=None, epilogue=EPI_LINEAR,
+         epi_alpha=LEAKY_ALPHA, aux=None):
+    """Cout = act(alpha * A @ B + bias) + beta * Cout for 2-D (possibly transposed) views; then, with epilogue SLOPE or
+    TANHGRAD, the data-gradient epilogue given `aux` (a tensor of Cout's shape, unit column stride): cape_gemm_ex."""
     M, N, K, a_rs, a_cs, b_rs, b_cs = _gemm_strides(A, B, Cout)
     with _Prof("gemm", tag):
-        check(tp.lib.cape_gemm(tp.h, M, N, K, _ptr(_f32(A)), a_rs, a_cs, _ptr(_f32(B)), b_rs, b_cs, _ptr(_f32(Cout)),
-                               Cout.stride(0), _ptr(bias), act, LEAKY_ALPHA, alpha, beta, _stream()))
+        if epilogue == EPI_LINEAR:
+            check(tp.lib.cape_gemm(tp.h, M, N, K, _ptr(_f32(A)), a_rs, a_cs, _ptr(_f32(B)), b_rs, b_cs,
+                                   _ptr(_f32(Cout)), Cout.stride(0), _ptr(bias), act, LEAKY_ALPHA, alpha, beta,
+                                   _stream()))
+            return
+        assert tuple(aux.shape) == (M, N) and (aux.stride(1) == 1 or N == 1)
+        check(tp.lib.cape_gemm_ex(tp.h, M, N, K, _ptr(_f32(A)), a_rs, a_cs, _ptr(_f32(B)), b_rs, b_cs, _ptr(_f32(Cout)),
+                                  Cout.stride(0), _ptr(bias), act, LEAKY_ALPHA, alpha, beta, epilogue, epi_alpha,
+                                  _ptr(_f32(aux)), aux.stride(0), _stream()))
 
 
 def cheb_call(tp, N, rows_out, ncols, terms, out, out2=None, cond=None, epilogue=EPI_LINEAR, act=ACT_NONE,

@@ -17,7 +17,7 @@ import torch
 from . import _lib
 from . import engine as E
 from . import topology as topo
-from .engine import (ACT_LEAKY, ACT_NONE, EPI_AFFINE, EPI_DUALMASK, EPI_LINEAR, ConvSite, Topology,
+from .engine import (ACT_LEAKY, ACT_NONE, EPI_AFFINE, EPI_DUALMASK, EPI_LINEAR, EPI_SLOPE, ConvSite, Topology,
                      act_bwd, axpy, cheb_call, cheb_dw, colsum, gemm)
 from .params import init_params, is_d_param, is_g_param, param_specs
 
@@ -481,9 +481,13 @@ class Dense:
         gemm(self.tp, x, self.W, out, bias=self.b, act=self.act,
              tag=(self.name + ":fwd", 4 * (M * (K + Nn) + K * Nn)))      # SURVEY 8(d): 4N(in+out) + 4 in*out
 
-    def bwd(self, x, out, dout, gtmp=None, dx=None, dx_beta=0.0, want_dw=True):
+    def bwd(self, x, out, dout, gtmp=None, dx=None, dx_beta=0.0, want_dw=True, pre_act=False, dx_epi=EPI_LINEAR,
+            dx_aux=None, dx_alpha=E.LEAKY_ALPHA):
+        """pre_act: dout is already the gradient w.r.t. the pre-activation (a consumer's epilogue ran the activation's
+        backward).  dx_epi / dx_aux / dx_alpha: the data-gradient epilogue of the dx product (cape_gemm_ex), applied
+        after the beta accumulation."""
         g = dout
-        if self.act != ACT_NONE:
+        if self.act != ACT_NONE and not pre_act:
             act_bwd(self.tp, dout, out, gtmp)
             g = gtmp
         N = g.shape[0]
@@ -491,7 +495,7 @@ class Dense:
             gemm(self.tp, x.t(), g, self.gW)
             gemm(self.tp, self.net.ones[:, :N], g, self.gb.view(1, -1))
         if dx is not None:
-            gemm(self.tp, g, self.W.t(), dx, beta=dx_beta)
+            gemm(self.tp, g, self.W.t(), dx, beta=dx_beta, epilogue=dx_epi, aux=dx_aux, epi_alpha=dx_alpha)
 
 
 class GNBlock:
@@ -675,8 +679,6 @@ class CapeNetwork:
         self.N = int(batch_size)
         self.ref_compat = bool(ref_compat)
         c = self.cfg
-        if not c["use_res_block_dec"] or c["reduce_dim"] <= 0:
-            raise NotImplementedError("the plain decoder (use_res_block_dec=0) and reduce_dim=0 are not built")
         if c["optimizer"] not in ("sgd", "adam"):
             raise NotImplementedError("optimizer must be 'sgd' (momentum) or 'adam' (lib/models.py:449-453)")
         # the encoder / discriminator activation (forward act, backward epilogue, alpha) and the reconstruction loss
@@ -723,9 +725,16 @@ class CapeNetwork:
 
         # ---- sites -------------------------------------------------------------------------------------
         nl = len(F)
+        # reduce_dim 0 (models.py:549-552,585-589): no 1x1 convs, the FC layers read the last encoder layer's output and
+        # write the first decoder layer's input directly
+        self.rd0 = c["reduce_dim"] <= 0
         if self.reorder:
             og = topo.level_orders(L[0], D[:nl])
             od = topo.level_orders(L_d[0], D_d)
+            if self.rd0:
+                # the 1x1 convs carried the permutation at the FC boundary: without them the coarsest level stays in the
+                # reference numbering (folded into the last encoder layer's output and the first decoder layer's input)
+                og[nl] = None
         else:
             og, od = [None] * (nl + 1), [None] * (len(D_d) + 1)
         self.order_g, self.order_d = og, od
@@ -746,11 +755,11 @@ class CapeNetwork:
                                           bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=self.brelu[0], need_dx=(i > 0),
                                           maxN=N, name="enc/conv%d" % (i + 1)))
             fin = F[i]
-        red = specs["generator/encoder/1x1-conv/weights"][1]
+        red = F[-1] if self.rd0 else specs["generator/encoder/1x1-conv/weights"][1]
         self.red = red
-        self.enc_1x1 = ChebLayer(self, ConvSite(tp, L[-1], 1, order_in=og[nl]), F[-1], 0, red,
-                                 w("generator/encoder/1x1-conv/weights"),
-                                 g("generator/encoder/1x1-conv/weights"), maxN=N, name="enc/1x1")
+        self.enc_1x1 = None if self.rd0 else ChebLayer(self, ConvSite(tp, L[-1], 1, order_in=og[nl]), F[-1], 0, red,
+                                                       w("generator/encoder/1x1-conv/weights"),
+                                                       g("generator/encoder/1x1-conv/weights"), maxN=N, name="enc/1x1")
         flat = self.p[-1] * red
         self.flat = flat
         dn = lambda s, act=ACT_NONE: Dense(self, w(s + "/dense/kernel").view(specs[s + "/dense/kernel"]),
@@ -758,14 +767,26 @@ class CapeNetwork:
                                            g(s + "/dense/bias"), act, name=s.split("/", 1)[-1])
         self.fc_mean, self.fc_var = dn("generator/encoder/fc_mean"), dn("generator/encoder/fc_var")
         self.dec_fc1 = dn("generator/decoder/fc1", ACT_LEAKY)
-        self.dec_1x1 = ChebLayer(self, ConvSite(tp, L[-1], 1, order_out=og[nl]), red, 0, F[-1],
-                                 w("generator/decoder/1x1-conv/weights"),
-                                 g("generator/decoder/1x1-conv/weights"), maxN=N, name="dec/1x1")
+        self.dec_1x1 = None if self.rd0 else ChebLayer(self, ConvSite(tp, L[-1], 1, order_out=og[nl]), red, 0, F[-1],
+                                                       w("generator/decoder/1x1-conv/weights"),
+                                                       g("generator/decoder/1x1-conv/weights"), maxN=N, name="dec/1x1")
         self.dec = []
-        self.affine = bool(c["affine"])
+        # decoder family: the plain decoder (udn, models.py:173-191) whenever use_res_block_dec is off, whatever
+        # `affine` says (:597-603); else affine or GroupNorm residual blocks
+        self.plain_dec = not c["use_res_block_dec"]
+        self.affine = bool(c["affine"]) and not self.plain_dec
         fin = F[-1]
         for i in range(nl):
-            if self.affine:
+            if self.plain_dec:
+                # unpool + Chebyshev conv on the finer level + bias + the model's brelu (tanh included), one ChebLayer
+                # whose condition channels enter through the epilogue (rowsum(U) y, never materialised)
+                Fo = F[-i - 1]
+                site = ConvSite(tp, L[-i - 2], K[-i - 1], U=U[-i - 1], order_in=og[nl - i], order_out=og[nl - i - 1])
+                sc = "generator/decoder/decoder_conv%d" % (i + 1)
+                self.dec.append(ChebLayer(self, site, fin, Cc, Fo, w(sc + "/weights"), g(sc + "/weights"),
+                                          bias=w(sc + "/bias"), gbias=g(sc + "/bias"), act=self.brelu[0], maxN=N,
+                                          name="dec/conv%d" % (i + 1)))
+            elif self.affine:
                 Fo = F[-i - 1] // 2
                 site = ConvSite(tp, L[-i - 2], K[-i - 1], U=U[-i - 1], order_in=og[nl - i], order_out=og[nl - i - 1])
                 sc = "generator/decoder/decoder_resblock_affine%d" % (i + 1)
@@ -823,14 +844,15 @@ class CapeNetwork:
         self.cc_h = z(2 * N, specs["condition_clo_label/fc1/dense/kernel"][1]) if self.c_clo2 else None
         enc_shape = [(l.conv2.site.rows_out, l.Fo) if self.enc_res else (l.site.rows_out, l.Fout) for l in self.enc]
         self.enc_act = [z(N, *s) for s in enc_shape]
-        self.enc_red = z(N, self.p[-1], red)
+        # the FC layers' input: the 1x1 conv's output, or (reduce_dim 0) the last encoder layer's output itself
+        self.enc_red = self.enc_act[-1] if self.rd0 else z(N, self.p[-1], red)
         self.z_mean, self.z_logvar = z(N, nz), z(N, nz)
         self.z_total = z(N, nz + Cc)
         self.dec_fc = z(N, flat)
-        self.dec_h0 = z(N, self.p[-1], F[-1])
-        if self.affine:
+        self.dec_h0 = self.dec_fc.view(N, self.p[-1], F[-1]) if self.rd0 else z(N, self.p[-1], F[-1])
+        if self.affine or self.plain_dec:
             self.dec_act = [z(N, l.site.rows_out, l.Fout) for l in self.dec]
-            self.dec_rg = [z(N, l.site.rows_out, l.Fout) for l in self.dec]
+            self.dec_rg = [z(N, l.site.rows_out, l.Fout) for l in self.dec] if self.affine else []
         else:
             self.dec_act = [z(N, b.rows, b.Fo) for b in self.dec]
             self.dec_rg = []
@@ -844,13 +866,21 @@ class CapeNetwork:
         self.d_ycat = z(N, Cc)
         self.g_dec = [torch.zeros_like(a) for a in self.dec_act]             # d out of each block
         self.g_dec_m = [torch.zeros_like(a) for a in self.dec_act] if self.affine else []   # masked (graph-conv branch)
-        self.g_dec_h0 = z(N, self.p[-1], F[-1])
         self.g_dec_fc = z(N, flat)
-        self.g_dec_fc_t = z(N, flat)
+        self.g_dec_fc_t = z(N, flat)            # d fc1's pre-activation
+        if not self.rd0:
+            self.g_dec_h0 = z(N, self.p[-1], F[-1])
+        elif isinstance(self.dec[0], ChebLayer):
+            # the first decoder layer's data gradient runs fc1's leaky-ReLU backward in its epilogue
+            self.g_dec_h0 = self.g_dec_fc_t.view(N, self.p[-1], F[-1])
+        else:
+            self.g_dec_h0 = self.g_dec_fc.view(N, self.p[-1], F[-1])
         self.g_z = z(N, nz)
         self.g_mean, self.g_logvar = z(N, nz), z(N, nz)
-        self.g_enc_red = z(N, self.p[-1], red)
         self.g_enc = [z(N, *s) for s in enc_shape]
+        # d (the FC layers' input); at reduce_dim 0 the FC data gradient runs the last encoder layer's activation
+        # backward in its epilogue and writes that layer's pre-activation gradient
+        self.g_enc_red = self.g_enc[-1] if self.rd0 else z(N, self.p[-1], red)
         self.g_cp_h, self.g_cp_t = z(N, h1), z(N, h1)
         self.g_cc_h = z(N, self.cc_h.shape[1]) if self.c_clo2 else None
         self.g_cc_t = z(N, self.cc_h.shape[1]) if self.c_clo2 else None
@@ -892,9 +922,10 @@ class CapeNetwork:
         self.prep_weights()
 
     def all_layers(self):
-        dec = self.dec if self.affine else [l for b in self.dec for l in b.layers()]
+        dec = self.dec if (self.affine or self.plain_dec) else [l for b in self.dec for l in b.layers()]
         enc = [l for b in self.enc for l in b.layers()] if self.enc_res else self.enc
-        return enc + [self.enc_1x1, self.dec_1x1] + dec + [self.dec_out] + self.disc + [self.disc_pred]
+        mid = [l for l in (self.enc_1x1, self.dec_1x1) if l is not None]
+        return enc + mid + dec + [self.dec_out] + self.disc + [self.disc_pred]
 
     def run_dw(self, fn):
         """Issue the weight-gradient launches `fn(topology)` of one layer: on the side stream (after everything
@@ -994,7 +1025,8 @@ class CapeNetwork:
         for l, a in zip(self.enc, self.enc_act):
             l.fwd(x, yc, a)
             x, yc = a, None
-        self.enc_1x1.fwd(x, None, self.enc_red)
+        if self.enc_1x1 is not None:
+            self.enc_1x1.fwd(x, None, self.enc_red)
         flat = self.enc_red.view(self.N, self.flat)
         self.fc_mean.fwd(flat, self.z_mean)
         self.fc_var.fwd(flat, self.z_logvar)
@@ -1010,11 +1042,16 @@ class CapeNetwork:
         ycat = self.ycat_g if ycat is None else ycat
         out = self.x_hat if out is None else out
         self.dec_fc1.fwd(z_total, self.dec_fc)
-        self.dec_1x1.fwd(self.dec_fc.view(self.N, self.p[-1], self.red), None, self.dec_h0)
+        if self.dec_1x1 is not None:
+            self.dec_1x1.fwd(self.dec_fc.view(self.N, self.p[-1], self.red), None, self.dec_h0)
         x = self.dec_h0
         if self.affine:
             for l, a, rg in zip(self.dec, self.dec_act, self.dec_rg):
                 l.fwd(x, ycat, a, out2=rg)
+                x = a
+        elif self.plain_dec:
+            for l, a in zip(self.dec, self.dec_act):
+                l.fwd(x, ycat, a)
                 x = a
         else:
             for b, a in zip(self.dec, self.dec_act):
@@ -1051,7 +1088,21 @@ class CapeNetwork:
         N, nl = self.N, len(self.dec)
         yc = self.ycat_g
         last = self.dec_act[-1]
-        if not self.affine:
+        # at reduce_dim 0 the first decoder layer reads fc1's leaky-ReLU output: a conv layer's data-gradient epilogue runs
+        # that activation's backward (g_dec_h0 is then d fc1's pre-activation), the GroupNorm block leaves it to fc1
+        first = dict(dx_epi=EPI_SLOPE, dx_aux=self.dec_h0, dx_alpha=E.LEAKY_ALPHA) if self.rd0 else {}
+        fc1_pre_act = self.rd0 and isinstance(self.dec[0], ChebLayer)
+        if self.plain_dec:
+            # every layer's data gradient runs the backward of the layer that produced its input (aux = that output)
+            _, epi, alpha = self.brelu
+            self.dec_out.bwd(last, yc, self.d_xhat, dx=self.g_dec[-1], dx_epi=epi, dx_aux=last, dx_alpha=alpha,
+                             dycat=self.d_ycat)
+            for i in range(nl - 1, 0, -1):
+                a = self.dec_act[i - 1]
+                self.dec[i].bwd(a, yc, self.g_dec[i], dx=self.g_dec[i - 1], dx_epi=epi, dx_aux=a, dx_alpha=alpha,
+                                dycat=self.d_ycat)
+            self.dec[0].bwd(self.dec_h0, yc, self.g_dec[0], dx=self.g_dec_h0, dycat=self.d_ycat, **first)
+        elif not self.affine:
             self.dec_out.bwd(last, yc, self.d_xhat, dx=self.g_dec[-1], dycat=self.d_ycat)
             for i in range(nl - 1, -1, -1):
                 x = self.dec_act[i - 1] if i > 0 else self.dec_h0
@@ -1059,17 +1110,22 @@ class CapeNetwork:
         else:
             self.dec_out.bwd(last, yc, self.d_xhat, dx=self.g_dec[-1], dx2=self.g_dec_m[-1], dx_epi=EPI_DUALMASK,
                              dx_aux=self.dec_rg[-1], dycat=self.d_ycat)
-        for i in range(nl - 1 if self.affine else -1, -1, -1):
-            x = self.dec_act[i - 1] if i > 0 else self.dec_h0
-            if i > 0:
-                self.dec[i].bwd(x, yc, self.g_dec_m[i], g_aff=self.g_dec[i], dx=self.g_dec[i - 1],
-                                dx2=self.g_dec_m[i - 1], dx_epi=EPI_DUALMASK, dx_aux=self.dec_rg[i - 1],
-                                dycat=self.d_ycat)
-            else:
-                self.dec[i].bwd(x, yc, self.g_dec_m[i], g_aff=self.g_dec[i], dx=self.g_dec_h0, dycat=self.d_ycat)
-        fcv = self.dec_fc.view(N, self.p[-1], self.red)
-        self.dec_1x1.bwd(fcv, None, self.g_dec_h0, dx=self.g_dec_fc.view(N, self.p[-1], self.red))
-        self.dec_fc1.bwd(self.z_total, self.dec_fc, self.g_dec_fc, gtmp=self.g_dec_fc_t)
+            for i in range(nl - 1, -1, -1):
+                x = self.dec_act[i - 1] if i > 0 else self.dec_h0
+                if i > 0:
+                    self.dec[i].bwd(x, yc, self.g_dec_m[i], g_aff=self.g_dec[i], dx=self.g_dec[i - 1],
+                                    dx2=self.g_dec_m[i - 1], dx_epi=EPI_DUALMASK, dx_aux=self.dec_rg[i - 1],
+                                    dycat=self.d_ycat)
+                else:
+                    self.dec[i].bwd(x, yc, self.g_dec_m[i], g_aff=self.g_dec[i], dx=self.g_dec_h0, dycat=self.d_ycat,
+                                    **first)
+        if self.dec_1x1 is not None:
+            fcv = self.dec_fc.view(N, self.p[-1], self.red)
+            self.dec_1x1.bwd(fcv, None, self.g_dec_h0, dx=self.g_dec_fc.view(N, self.p[-1], self.red))
+        if fc1_pre_act:
+            self.dec_fc1.bwd(self.z_total, self.dec_fc, self.g_dec_fc_t, pre_act=True)
+        else:
+            self.dec_fc1.bwd(self.z_total, self.dec_fc, self.g_dec_fc, gtmp=self.g_dec_fc_t)
         W = self.dec_fc1.W                     # [nz + Cc, flat]: rows [0,nz) latent code, rows [nz,..) condition (models.py:641)
         gemm(self.tp, self.g_dec_fc_t, W[:self.nz].t(), self.g_z)
         gemm(self.tp, self.g_dec_fc_t, W[self.nz:].t(), self.d_ycat, beta=1.0)
@@ -1083,13 +1139,17 @@ class CapeNetwork:
                                                    E._stream()))
         flat = self.enc_red.view(N, self.flat)
         gflat = self.g_enc_red.view(N, self.flat)
+        _, epi, alpha = self.brelu
+        # reduce_dim 0: the second product (beta = 1) ends the sum, so it runs the last encoder layer's activation
+        # backward in its epilogue and gflat is that layer's pre-activation gradient g_enc[-1]
+        last = dict(dx_epi=epi, dx_aux=flat, dx_alpha=alpha) if self.rd0 else {}
         self.fc_mean.bwd(flat, self.z_mean, self.g_mean, dx=gflat)
-        self.fc_var.bwd(flat, self.z_logvar, self.g_logvar, dx=gflat, dx_beta=1.0)
+        self.fc_var.bwd(flat, self.z_logvar, self.g_logvar, dx=gflat, dx_beta=1.0, **last)
         self._fc_reg(("generator/encoder/fc_mean", "generator/encoder/fc_var"))
         self._reduce_bucket("enc_fc")                       # 28 MB of gradients are final: all-reduce behind the conv backward
-        _, epi, alpha = self.brelu
-        self.enc_1x1.bwd(self.enc_act[-1], None, self.g_enc_red, dx=self.g_enc[-1], dx_epi=epi,
-                         dx_aux=self.enc_act[-1], dx_alpha=alpha)
+        if self.enc_1x1 is not None:
+            self.enc_1x1.bwd(self.enc_act[-1], None, self.g_enc_red, dx=self.g_enc[-1], dx_epi=epi,
+                             dx_aux=self.enc_act[-1], dx_alpha=alpha)
         yc = self.ycat_g if self.cond_enc else None
         dyc = self.d_ycat if self.cond_enc else None        # complete before cond_bwd (the small products flush first)
         for i in range(len(self.enc) - 1, 0, -1):
@@ -1146,7 +1206,7 @@ class CapeNetwork:
         self.arena.zero()
         self.losses.zero_()
         self.d_ycat.zero_()
-        if not self.affine:
+        if not (self.affine or self.plain_dec):
             self.PG.grad.zero_()          # group-norm gamma/beta gradients are accumulated by their kernels
         # forward: both condition batches at once, generator, discriminator on [real ; fake]
         self.cond_fwd(0, 2 * N)

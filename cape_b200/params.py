@@ -82,7 +82,13 @@ def param_specs(cfg, p, p_d):
     for i in range(len(F)):
         Fo = F[-i - 1]
         Kb = K[-i - 1]
-        if cfg["affine"]:
+        if not cfg["use_res_block_dec"]:
+            # udn (models.py:173-191, chosen at :597-603 whatever `affine` says): unpool, filter, brelu
+            sc = "generator/decoder/decoder_conv%d" % (i + 1)
+            s[sc + "/weights"] = (fin * Kb, Fo)
+            s[sc + "/bias"] = (1, 1, Fo)
+            fin = Fo + Cc
+        elif cfg["affine"]:
             sc = "generator/decoder/decoder_resblock_affine%d" % (i + 1)
             s[sc + "/graph_conv/weights"] = (fin * Kb, Fo // 2)
             s[sc + "/affine/weights"] = (fin, Fo // 2)

@@ -209,6 +209,19 @@ int cape_gemm(cape_topology* t, int M, int N, int K,
               float* c, int64_t c_rs,
               const float* bias, int act, float leaky_alpha, float alpha, float beta, void* stream);
 
+/* cape_gemm followed by a data-gradient epilogue of the conv kernels, applied last (after the beta accumulation):
+ *   CAPE_EPI_LINEAR    C as cape_gemm writes it (aux unread);
+ *   CAPE_EPI_SLOPE     C *= (aux > 0 ? 1 : epi_alpha)      (leaky ReLU / ReLU backward given the layer's output);
+ *   CAPE_EPI_TANHGRAD  C *= 1 - aux^2                      (tanh backward given the layer's output);
+ * aux(m, n) = aux[m*aux_rs + n], C's shape.  The FC layers' input gradient at reduce_dim 0 is this product: it is the
+ * gradient w.r.t. the last encoder layer's pre-activation, without a separate pass over the N x p*F tensor. */
+int cape_gemm_ex(cape_topology* t, int M, int N, int K,
+                 const float* a, int64_t a_rs, int64_t a_cs,
+                 const float* b, int64_t b_rs, int64_t b_cs,
+                 float* c, int64_t c_rs,
+                 const float* bias, int act, float leaky_alpha, float alpha, float beta,
+                 int epilogue, float epi_alpha, const float* aux, int64_t aux_rs, void* stream);
+
 /* Many small products in ONE launch: C_i = alpha_i * A_i.B_i (beta_i = 0) or C_i += alpha_i * A_i.B_i (beta_i = 1:
  * atomic, several items may add into the same C).  The bias / condition-channel gradients of a training step are ~80
  * products of [64 x 64]-sized operands; the step's schedule is static, so the caller collects them, builds the device

@@ -27,6 +27,13 @@
 // fastest, so the CTAs of one row tile run together and read its source rows from L2 rather than from HBM once per
 // column tile, and a CTA that starts late (the weight-gradient stream holding its SM) simply takes fewer tiles.
 //
+// A launch of more than 128 output columns runs WIDE tiles instead: 64 rows x 256 columns (128 per sum with two
+// accumulators), both consumers reading the same A chunk and each issuing its wgmma on its own column half, so each
+// gathered basis row feeds twice the columns.  Its 32-deep chunks span two 16-deep
+// stages (64-byte swizzle, four stages in the ring) and the two producer warpgroups fill alternate chunks, each
+// thread gathering two row pairs as above.  The plain-operand launches keep the 128-row tiles: their A operand is no
+// gather, and the wide tile made them slower (tools/conv_tile_cost.py).
+//
 // Every chunk's products go to a fresh register accumulator that is added to the running sum in fp32 with
 // round-to-nearest, so the tensor core's truncating accumulation chain is one chunk (12 MMAs) long instead of the whole
 // reduction: long reductions would otherwise drift from the fp64 truth by more than 1e-4.
@@ -53,25 +60,40 @@ constexpr int CONSUMER_THREADS = 256;
 constexpr int PRODUCER_REGS = 112;
 constexpr int CONSUMER_REGS = 144;
 constexpr int GATHER_PAIRS = 2;               // row pairs each producer thread gathers at once
-constexpr int A_TILE = BM * 128;              // 128 rows x 32 fp32
 constexpr int QS_MAX_FLOATS = 8192;           // condition vectors of the tile's samples and columns
 constexpr int BAR_BYTES = 256;                // the ring's mbarriers and tile slots
 constexpr int SMEM_MAX = 227 * 1024;          // dynamic shared memory per CTA on sm_90
 
+// BN: the tile's columns (per sum).  Up to 128 (64 with two accumulators) a tile is 128 rows x BN columns, each
+// consumer taking 64 rows; wider (BN = 256, or 128 with two accumulators) it is a WIDE tile of 64 rows, both consumers
+// reading the same A chunk and each taking its own column half: the same MMAs and accumulator registers per consumer
+// (CN = 128 or 64 columns) for half the gathered rows.  A stage holds KS k of the tile's
+// A and B operands, hi and lo, in tile rows of KS * 4 bytes: 32 k with the 128-byte swizzle, or with WIDE 16 k with
+// the 64-byte swizzle (a 32-deep stage of the wide tile would leave room for only two), so that a wide 32-deep
+// chunk spans SUB = 2 consecutive stages.
 template <int BN, bool DUAL>
 struct ConvCfg {
-  static constexpr int B_TILE = BN * 128;
+  static constexpr bool WIDE = BN > (DUAL ? 64 : 128);
+  static constexpr int CN = WIDE ? BN / 2 : BN;       // the columns (per sum) of each consumer's wgmma
+  static constexpr int ROWS = WIDE ? 64 : BM;
+  static constexpr int COLS = BN;
+  static constexpr int KS = WIDE ? 16 : BK;
+  static constexpr int SUB = BK / KS;
+  static constexpr int ROW_BYTES = KS * 4;
+  static constexpr int PT = PRODUCER_THREADS / SUB;   // producer threads per chunk
+  static constexpr int A_TILE = ROWS * ROW_BYTES;
+  static constexpr int B_TILE = COLS * ROW_BYTES;
   static constexpr int STAGE = 2 * A_TILE + (DUAL ? 4 : 2) * B_TILE;
   // as many stages (up to 4) as fit beside the largest condition-vector buffer
   static constexpr int FIT = (SMEM_MAX - 1024 - BAR_BYTES - QS_MAX_FLOATS * 4) / STAGE;
   static constexpr int STAGES = FIT < 4 ? FIT : 4;
   static constexpr int RING = STAGES * STAGE;
-  static_assert(STAGES >= 3, "the ring needs at least three stages");
+  static_assert(STAGES >= 3 && STAGES % SUB == 0, "the ring needs at least three stages, whole chunks");
   static_assert(3 * STAGES * 8 + STAGES * 4 <= BAR_BYTES, "mbarrier area too small");
 };
 
 // TMA descriptors of the terms' K-major weight copies, encoded at launch: w[t][0] maps wT and w[t][1] w2T of term t,
-// each as a [ncols x F] tensor (row stride wT_stride) read in boxes of 32 k x BN columns with the 128-byte swizzle,
+// each as a [ncols x F] tensor (row stride wT_stride) read in boxes of KS k x COLS columns with the stage's swizzle,
 // the layout of the stage's weight tiles; the zero fill beyond F and ncols pads the last chunk and column tile
 struct WeightMaps {
   CUtensorMap w[CAPE_MAX_TERMS][2];
@@ -133,8 +155,11 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
                                                                   int max_samples, int ncol_tiles, int ntiles,
                                                                   unsigned* counter) {
   using Cfg = ConvCfg<BN, DUAL>;
+  constexpr bool WIDE = Cfg::WIDE;
   constexpr int S = Cfg::STAGES;
-  constexpr int NA = BN / 2;                  // accumulator registers per consumer thread
+  constexpr int SUB = Cfg::SUB;
+  constexpr int CN = Cfg::CN;
+  constexpr int NA = CN / 2;                  // accumulator registers per consumer thread
   extern __shared__ uint8_t smem_raw[];
   char* smem = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + Cfg::RING);
@@ -153,7 +178,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
 
   if (tid == 0) {
     for (int s = 0; s < S; ++s) {
-      mbar_init(&full[s], PRODUCER_THREADS);  // every producer thread
+      mbar_init(&full[s], Cfg::PT);           // every producer thread of the chunk
       mbar_init(&empty[s], 8);                // one lane per consumer warp
       mbar_init(&wfull[s], 1);                // the producer that issues the stage's weight loads
     }
@@ -164,11 +189,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   if (tid < PRODUCER_THREADS) {
     // =========================== producers ===========================
     setmaxnreg_dec<PRODUCER_REGS>();
-    // 8 threads per 128-byte tile row (one float4 of k each), 32 row slots; rows rs + 32 i, gathered in the pairs
-    // (rs, rs + 32) and (rs + 64, rs + 96): the row mapping of the SIMT kernels, so each row's taps add in their order
-    const int l8 = tid & 7, rs = tid >> 3;
-    constexpr int ROWS[4] = {0, 32, 64, 96};
-    uint32_t it = 0;                          // the CTA's running chunk count: ring stage it % S, phase (it / S) & 1
+    // 8 threads per row of a 32-deep chunk (one float4 of k each), rows rs + RSTEP i, gathered in the pairs
+    // (rs, rs + RSTEP) and (rs + 2 RSTEP, rs + 3 RSTEP): with 128-row tiles both producer warpgroups fill every chunk,
+    // with the 64-row WIDE tiles each fills every other one (its own stages), so that a thread still gathers two
+    // pairs of rows at once.  The row mapping of the SIMT kernels: each row's taps add in their order.
+    const int pw = WIDE ? wg : 0;             // the producer warpgroup, for WIDE: it fills the chunks of its parity
+    const int pt = tid - pw * Cfg::PT;        // the thread among the chunk's producers
+    const int l8 = pt & 7, rs = pt >> 3;
+    constexpr int RSTEP = Cfg::ROWS / 4;
+    uint32_t it = 0;                          // the CTA's running stage count: ring stage it % S, phase (it / S) & 1
     unsigned next = 0;
     if (tid == 0) next = atomicAdd(counter, 1u);
     for (;;) {
@@ -177,42 +206,53 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
       if (tid == 0) tile_slot[it % S] = next < (unsigned)ntiles ? (int)next : -1;
       named_bar_sync(2, PRODUCER_THREADS);
       const int tile = tile_slot[it % S];     // not rewritten before the consumers have released this stage
+      const bool mine0 = (int)((it / SUB) & 1) == pw || !WIDE;   // this warpgroup fills the tile's first chunk
       if (tile < 0) {                         // no more tiles
         if (tid == 0 && next == (unsigned)ntiles + gridDim.x - 1) *counter = 0u;   // the launch's last ticket
-        mbar_arrive(&full[it % S]);
+        if (mine0) mbar_arrive(&full[it % S]);
         return;
       }
       if (tid == 0) next = atomicAdd(counter, 1u);   // the following tile's ticket, in flight during this tile
       const int ct = tile % ncol_tiles;
-      const long long row0 = (long long)(tile / ncol_tiles) * BM;
-      const int col0 = ct * BN;
+      const long long row0 = (long long)(tile / ncol_tiles) * Cfg::ROWS;
+      const int col0 = ct * Cfg::COLS;
       int rn[4], rr[4];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        const long long R = row0 + rs + ROWS[i];
+        const long long R = row0 + rs + RSTEP * i;
         if (R < p.total_rows) { rn[i] = (int)(R / p.rows_out); rr[i] = (int)(R % p.rows_out); }
         else { rn[i] = -1; rr[i] = 0; }
       }
       const bool do_stash = ct == 0;          // one column tile writes the basis copies
       int t = 0, f0 = 0;
-      for (int j = 0; j < nchunks; ++j, ++it) {
-        const int stage = it % S;
-        mbar_wait(&empty[stage], ((it / S) & 1) ^ 1);
-        char* a_hi = smem + (size_t)stage * Cfg::STAGE;
-        char* a_lo = a_hi + A_TILE;
-        char* b_hi = a_lo + A_TILE;
-        char* b_lo = b_hi + Cfg::B_TILE;
+      for (int j = 0; j < nchunks; ++j, it += SUB) {
         const TermDev& tm = p.terms[t];
+        if (WIDE && (int)((it / SUB) & 1) != pw) {   // the other warpgroup's chunk
+          f0 += BK;
+          if (f0 >= tm.F) { f0 = 0; ++t; }
+          continue;
+        }
+#pragma unroll
+        for (int u = 0; u < SUB; ++u) mbar_wait(&empty[(it + u) % S], (((it + u) / S) & 1) ^ 1);
         const int f = f0 + l8 * 4;
         // the weight chunk first, by TMA into the hi tiles: it lands while the gather runs
         const bool has2 = DUAL && tm.w2T != nullptr;
-        if (tid == 0) {
-          mbar_arrive_expect_tx(&wfull[stage], (has2 ? 2 : 1) * Cfg::B_TILE);
-          tma_load_2d(b_hi, &maps.w[t][0], f0, col0, &wfull[stage]);
-          if (has2) tma_load_2d(b_lo + Cfg::B_TILE, &maps.w[t][1], f0, col0, &wfull[stage]);
-        }
+        if (pt == 0) {
 #pragma unroll
-        for (int h = 0; h < 2 / GATHER_PAIRS; ++h) {  // GATHER_PAIRS pairs (ROWS[2q], ROWS[2q + 1]) at a time
+          for (int u = 0; u < SUB; ++u) {
+            const int stage = (it + u) % S;
+            char* b_hi = smem + (size_t)stage * Cfg::STAGE + 2 * Cfg::A_TILE;
+            mbar_arrive_expect_tx(&wfull[stage], (has2 ? 2 : 1) * Cfg::B_TILE);
+            tma_load_2d(b_hi, &maps.w[t][0], f0 + u * Cfg::KS, col0, &wfull[stage]);
+            if (has2) tma_load_2d(b_hi + 2 * Cfg::B_TILE, &maps.w[t][1], f0 + u * Cfg::KS, col0, &wfull[stage]);
+          }
+        }
+        // this thread's k go to the chunk's stage l8 / (8 / SUB), 16-byte chunk l8 % (8 / SUB) of its tile rows
+        char* a_hi = smem + (size_t)((it + l8 / (8 / SUB)) % S) * Cfg::STAGE;
+        char* a_lo = a_hi + Cfg::A_TILE;
+        const int kc = l8 % (8 / SUB);
+#pragma unroll
+        for (int h = 0; h < 2 / GATHER_PAIRS; ++h) {  // GATHER_PAIRS pairs (rows 2q, 2q + 1) at a time
           constexpr int NP = GATHER_PAIRS;
           float4 va[NP], vb[NP];
 #pragma unroll
@@ -246,28 +286,35 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
               const int i = 2 * (h * NP + q) + e;
               float4 v = e == 0 ? va[q] : vb[q];
               if (rn[i] < 0) v = make_float4(0.f, 0.f, 0.f, 0.f);
-              const int row = rs + ROWS[i];
+              const int row = rs + RSTEP * i;
               if (f < tm.F && tm.stash != nullptr && do_stash && rn[i] >= 0)   // basis rows for the weight gradient
                 *reinterpret_cast<float4*>(tm.stash + (size_t)(row0 + row) * tm.stash_stride + f) = v;
-              split_store4(v, a_hi, a_lo, (uint32_t)(row * 128 + ((l8 ^ (row & 7)) << 4)));
+              const int sw = WIDE ? (row >> 1) & 3 : row & 7;
+              split_store4(v, a_hi, a_lo, (uint32_t)(row * Cfg::ROW_BYTES + ((kc ^ sw) << 4)));
             }
           }
         }
         // the weight chunk, split in place: hi = tf32_hi(w), lo = w - hi (zeros for a term without w2T)
-        mbar_wait(&wfull[stage], (it / S) & 1);
 #pragma unroll
-        for (int i = 0; i < BN / 32; ++i) {
-          const int cl = rs + 32 * i;
-          const uint32_t off = (uint32_t)(cl * 128 + ((l8 ^ (cl & 7)) << 4));
-          split_store4(*reinterpret_cast<const float4*>(b_hi + off), b_hi, b_lo, off);
-          if (DUAL) {
-            char* b2_hi = b_lo + Cfg::B_TILE;
-            const float4 v2 = has2 ? *reinterpret_cast<const float4*>(b2_hi + off) : make_float4(0.f, 0.f, 0.f, 0.f);
-            split_store4(v2, b2_hi, b2_hi + Cfg::B_TILE, off);
+        for (int u = 0; u < SUB; ++u) {
+          const int stage = (it + u) % S;
+          char* b_hi = smem + (size_t)stage * Cfg::STAGE + 2 * Cfg::A_TILE;
+          char* b_lo = b_hi + Cfg::B_TILE;
+          mbar_wait(&wfull[stage], ((it + u) / S) & 1);
+#pragma unroll
+          for (int i = 0; i < Cfg::B_TILE / 16 / Cfg::PT; ++i) {   // the split is elementwise: any float4 order
+            const uint32_t off = (uint32_t)((pt + Cfg::PT * i) * 16);
+            split_store4(*reinterpret_cast<const float4*>(b_hi + off), b_hi, b_lo, off);
+            if (DUAL) {
+              char* b2_hi = b_lo + Cfg::B_TILE;
+              const float4 v2 = has2 ? *reinterpret_cast<const float4*>(b2_hi + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+              split_store4(v2, b2_hi, b2_hi + Cfg::B_TILE, off);
+            }
           }
         }
         fence_proxy_async();                  // generic-proxy smem writes -> visible to the tensor core's (async) proxy
-        mbar_arrive(&full[stage]);
+#pragma unroll
+        for (int u = 0; u < SUB; ++u) mbar_arrive(&full[(it + u) % S]);
         f0 += BK;
         if (f0 >= tm.F) { f0 = 0; ++t; }
       }
@@ -279,6 +326,9 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
   const int cw = wg - 2, ctid = tid - PRODUCER_THREADS;
   const EpiParams& e = p.epi;
   const bool use_aux = epi_reads_aux(e.epilogue);
+  // this consumer's share of a stage: its 64 rows of A, or with WIDE its CN-column half of B
+  const uint32_t a_off = WIDE ? 0u : (uint32_t)(cw * 64 * Cfg::ROW_BYTES);
+  const uint32_t b_off = 2 * Cfg::A_TILE + (WIDE ? (uint32_t)(cw * CN * Cfg::ROW_BYTES) : 0u);
   uint32_t it = 0;                            // as the producers' count
   for (;;) {
     mbar_wait(&full[it % S], (it / S) & 1);   // the tile's first chunk carries its index
@@ -287,24 +337,30 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
 
     // one chunk accumulator for both running sums where two would not fit beside them (DUAL, BN = 64): the second
     // sum's MMAs then wait for the first one's add
-    constexpr bool ONE_PART = DUAL && BN == 64;
+    constexpr bool ONE_PART = DUAL && CN == 64;
     float acc0[NA], acc1[DUAL ? NA : 1], part0[NA], part1[DUAL && !ONE_PART ? NA : 1];
 #pragma unroll
     for (int i = 0; i < NA; ++i) { acc0[i] = 0.f; if (DUAL) acc1[i] = 0.f; }
 
-    for (const uint32_t end = it + nchunks; it != end; ++it) {
-      const int stage = it % S;
-      mbar_wait(&full[stage], (it / S) & 1);
-      const uint32_t a_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + (uint32_t)(cw * 64 * 128);
-      const uint32_t a_lo = a_hi + A_TILE;
-      const uint32_t b_hi = smem_u32(smem + (size_t)stage * Cfg::STAGE) + 2 * A_TILE;
-      const uint32_t b_lo = b_hi + Cfg::B_TILE;
+    for (const uint32_t end = it + nchunks * SUB; it != end; it += SUB) {
+      // the chunk's MMAs for one sum (second = the w2 tiles) into d, a fresh accumulator, in the order of its k-steps
+      auto mma_sum = [&](float (&d)[NA], bool second) {
+#pragma unroll
+        for (int u = 0; u < SUB; ++u) {
+          const uint32_t base = smem_u32(smem + (size_t)((it + u) % S) * Cfg::STAGE);
+          const uint32_t b_hi = base + b_off + (second ? 2 * Cfg::B_TILE : 0);
+          mma3_chunk<CN, Cfg::KS / 8>(d, base + a_off, base + a_off + Cfg::A_TILE, b_hi, b_hi + Cfg::B_TILE,
+                                      u == 0 ? 0 : 1);
+        }
+      };
+#pragma unroll
+      for (int u = 0; u < SUB; ++u) mbar_wait(&full[(it + u) % S], ((it + u) / S) & 1);
       wgmma_fence();
       fence_acc(part0);
-      mma3_chunk<BN>(part0, a_hi, a_lo, b_hi, b_lo, 0);
+      mma_sum(part0, false);
       if constexpr (DUAL && !ONE_PART) {
         fence_acc(part1);
-        mma3_chunk<BN>(part1, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
+        mma_sum(part1, true);
       }
       wgmma_commit();
       wgmma_wait_all();
@@ -314,11 +370,14 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
         for (int i = 0; i < NA; ++i) acc0[i] += part0[i];
         wgmma_fence();
         fence_acc(part0);
-        mma3_chunk<BN>(part0, a_hi, a_lo, b_lo + Cfg::B_TILE, b_lo + 2 * Cfg::B_TILE, 0);
+        mma_sum(part0, true);
         wgmma_commit();
         wgmma_wait_all();
       }
-      if ((tid & 31) == 0) mbar_arrive(&empty[stage]);   // this warp's MMAs have read the stage (and its tile slot)
+      if ((tid & 31) == 0) {                  // this warp's MMAs have read the chunk's stages (and the tile slot)
+#pragma unroll
+        for (int u = 0; u < SUB; ++u) mbar_arrive(&empty[(it + u) % S]);
+      }
       fence_acc(part0);
 #pragma unroll
       for (int i = 0; i < NA; ++i) (ONE_PART ? acc1 : acc0)[i] += part0[i];
@@ -331,13 +390,15 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
 
     // the tile's coordinates only now, so that they take no registers beside the accumulators in the loop above
     const int ct = tile % ncol_tiles;
-    const long long row0 = (long long)(tile / ncol_tiles) * BM;
-    const int col0 = ct * BN;
+    const long long row0 = (long long)(tile / ncol_tiles) * Cfg::ROWS;
+    const int tcol0 = ct * Cfg::COLS;
+    const int col0 = tcol0 + (WIDE ? cw * CN : 0);   // this consumer's first column
     // condition broadcast vectors of this tile
     const int n_first = (int)(row0 / p.rows_out);
     if (p.nslots > 0) {
       named_bar_sync(1, CONSUMER_THREADS);    // the previous tile's epilogue has read qs
-      stage_cond<16>(p, qs, n_first, min(max_samples, p.N - n_first), col0, BN, p.ncols, ctid, CONSUMER_THREADS);
+      stage_cond<16>(p, qs, n_first, min(max_samples, p.N - n_first), tcol0, Cfg::COLS, p.ncols, ctid,
+                     CONSUMER_THREADS);
       named_bar_sync(1, CONSUMER_THREADS);    // qs complete
     }
 
@@ -346,7 +407,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
     // wide tile could end up indexed at run time (in local memory)
     auto row_epilogue = [&](auto h_const) {
       constexpr int h = decltype(h_const)::value;
-      const int lrow = cw * 64 + frag_row(wt, 2 * h);
+      const int lrow = (WIDE ? 0 : cw * 64) + frag_row(wt, 2 * h);
       const long long R = row0 + lrow;
       if (R >= p.total_rows) return;
       const int n = (int)(R / p.rows_out), r = (int)(R % p.rows_out);
@@ -355,7 +416,7 @@ __global__ void __launch_bounds__(CONV_THREADS, 1) conv_wg_kernel(const __grid_c
       // around the unrolled columns, so that the accumulators are only ever indexed by constants
       for (int slot = 0; slot < p.nslots; ++slot) {
         const float coef = cond_coef(p.terms[p.slot_term[slot]].op, r);
-        const float* q = cond_vec(qs, n - n_first, slot, p.nslots, BN) + frag_col(wt, 0);
+        const float* q = cond_vec(qs, n - n_first, slot, p.nslots, Cfg::COLS) + (col0 - tcol0) + frag_col(wt, 0);
         if (p.slot_acc[slot] == 0) {
 #pragma unroll
           for (int g = 0; g < NA / 4; ++g) {
@@ -421,8 +482,9 @@ PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
   return fn;
 }
 
-// wT (row c at wT + c * stride, F valid k) as a [ncols x F] tensor in boxes of 32 k x BN columns
-int encode_weight_map(CUtensorMap* m, const float* wT, int F, int stride, int ncols, int bn) {
+// wT (row c at wT + c * stride, F valid k) as a [ncols x F] tensor in boxes of ks k x cols columns, ks = 32 with the
+// 128-byte swizzle or 16 with the 64-byte swizzle
+int encode_weight_map(CUtensorMap* m, const float* wT, int F, int stride, int ncols, int ks, int cols) {
   const auto encode = tensor_map_encoder();
   if (encode == nullptr) {
     set_error("conv_wg_kernel: cuTensorMapEncodeTiled is not available from the CUDA driver");
@@ -430,10 +492,11 @@ int encode_weight_map(CUtensorMap* m, const float* wT, int F, int stride, int nc
   }
   const cuuint64_t dims[2] = {(cuuint64_t)F, (cuuint64_t)ncols};
   const cuuint64_t strides[1] = {(cuuint64_t)stride * sizeof(float)};
-  const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)bn};
+  const cuuint32_t box[2] = {(cuuint32_t)ks, (cuuint32_t)cols};
   const cuuint32_t estrides[2] = {1, 1};
   const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(wT), dims, strides, box, estrides,
-                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE,
+                            ks == BK ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("conv_wg_kernel: cuTensorMapEncodeTiled failed with CUresult " + std::to_string((int)r));
@@ -449,22 +512,23 @@ int launch_conv_inst(const cape_topology* t, const ConvParams& p, cudaStream_t s
   memset(&maps, 0, sizeof(maps));
   for (int i = 0; i < p.nterms; ++i) {
     const TermDev& tm = p.terms[i];
-    if (encode_weight_map(&maps.w[i][0], tm.wT, tm.F, tm.wT_stride, p.ncols, BN) != 0) return -2;
+    if (encode_weight_map(&maps.w[i][0], tm.wT, tm.F, tm.wT_stride, p.ncols, Cfg::KS, Cfg::COLS) != 0) return -2;
     if (DUAL && tm.w2T != nullptr &&
-        encode_weight_map(&maps.w[i][1], tm.w2T, tm.F, tm.w2T_stride, p.ncols, BN) != 0)
+        encode_weight_map(&maps.w[i][1], tm.w2T, tm.F, tm.w2T_stride, p.ncols, Cfg::KS, Cfg::COLS) != 0)
       return -2;
   }
-  const int max_samples = (int)max_tile_samples(BM, p.rows_out);
-  const int smem = 1024 + Cfg::RING + BAR_BYTES + max_samples * p.nslots * BN * 4;
+  const int max_samples = (int)max_tile_samples(Cfg::ROWS, p.rows_out);
+  const int smem = 1024 + Cfg::RING + BAR_BYTES + max_samples * p.nslots * Cfg::COLS * 4;
   static bool configured = false;
   if (!configured) {
-    CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL, PASS, TANH>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    CAPE_CHECK_CUDA(cudaFuncSetAttribute(conv_wg_kernel<BN, DUAL, PASS, TANH>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          1024 + Cfg::RING + BAR_BYTES + QS_MAX_FLOATS * 4));
     configured = true;
   }
   // tiles numbered with the column tiles fastest; one persistent CTA per SM (or per tile, if fewer)
-  const int ncol_tiles = (p.ncols + BN - 1) / BN;
-  const long long ntiles = (p.total_rows + BM - 1) / BM * ncol_tiles;
+  const int ncol_tiles = (p.ncols + Cfg::COLS - 1) / Cfg::COLS;
+  const long long ntiles = (p.total_rows + Cfg::ROWS - 1) / Cfg::ROWS * ncol_tiles;
   if (ntiles + t->sm_count >= (1LL << 31)) {
     set_error("conv_wg_kernel: too many tiles");
     return -1;
@@ -485,17 +549,17 @@ int launch_conv(const cape_topology* t, const ConvParams& p, cudaStream_t st) {
   return launch_conv_inst<BN, DUAL, PASS, false>(t, p, st);
 }
 
-// column tile width: the whole output row up to 128 columns (64 with two accumulators), so that the running sums and
-// the chunk accumulators fit the registers
+// column tile width of the 128-row tiles: the whole output row up to 128 columns (64 with two accumulators), so that
+// the running sums and the chunk accumulators fit the registers
 int pick_bn(int ncols, bool dual) {
   if (ncols <= 32) return 32;
   if (ncols <= 64 || dual) return 64;
   return 128;
 }
 
-// false if the condition vectors of a tile would not fit the staging buffer
-bool qs_fits(const ConvParams& p, int bn) {
-  return max_tile_samples(BM, p.rows_out) * p.nslots * bn <= QS_MAX_FLOATS;
+// false if the condition vectors of a tile of `rows` x `cols` would not fit the staging buffer
+bool qs_fits(const ConvParams& p, int rows, int cols) {
+  return max_tile_samples(rows, p.rows_out) * p.nslots * cols <= QS_MAX_FLOATS;
 }
 
 }  // namespace
@@ -520,13 +584,18 @@ int launch_ellconv_tc(const cape_topology* t, const ConvParams& p, bool dual, cu
     if (!p.terms[i].vec) return 0;
   if (kred < 64) return 0;                       // tiny reductions: the SIMT kernel is as good and simpler
   const int bn = pick_bn(p.ncols, dual);
-  if (!qs_fits(p, bn)) return 0;
+  // an output wider than 128 columns: WIDE tiles of 64 rows x 2 bn columns, which gather each basis chunk once for
+  // twice the columns (dual outputs of 128 columns keep the 128-row tiles of 64 columns)
+  const bool wide = p.ncols > 128 && qs_fits(p, 64, 2 * bn);
+  if (!wide && !qs_fits(p, BM, bn)) return 0;
   if (p.npass > 0) {                             // the encoder's residual blocks: single accumulator
     if (dual) return 0;
+    if (wide) return launch_conv<256, false, true>(t, p, st);
     if (bn == 32) return launch_conv<32, false, true>(t, p, st);
     if (bn == 64) return launch_conv<64, false, true>(t, p, st);
     return launch_conv<128, false, true>(t, p, st);
   }
+  if (wide) return dual ? launch_conv<128, true>(t, p, st) : launch_conv<256, false>(t, p, st);
   if (dual) return bn == 32 ? launch_conv<32, true>(t, p, st) : launch_conv<64, true>(t, p, st);
   if (bn == 32) return launch_conv<32, false>(t, p, st);
   if (bn == 64) return launch_conv<64, false>(t, p, st);
@@ -550,7 +619,7 @@ int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaS
   for (int s = 0; s < p.nslots; ++s)
     if (p.slot_acc[s] != 0) return 0;
   const int bn = pick_bn(p.ncols, false);
-  if (!qs_fits(p, bn)) return 0;
+  if (!qs_fits(p, BM, bn)) return 0;
   if (bn == 32) return launch_conv<32, false>(t, p, st);
   if (bn == 64) return launch_conv<64, false>(t, p, st);
   return launch_conv<128, false>(t, p, st);

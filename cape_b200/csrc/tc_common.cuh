@@ -4,7 +4,8 @@
 // Operand tiles are K-major with the 128-byte swizzle: one tile row holds 32 consecutive k (128 bytes), 16-byte chunk
 // j of row m sits at chunk j ^ (m & 7), rows follow each other every 128 bytes (8-row groups of 1024 bytes).  Tiles
 // start at 1024-byte boundaries, so a wgmma descriptor addresses the k-step ks (8 tf32 = 32 bytes) of a tile by adding
-// 32 * ks bytes to the start address.
+// 32 * ks bytes to the start address.  The wide tiles of conv_wg_kernel hold 16 k per row instead, with the 64-byte
+// swizzle: chunk j of row m at chunk j ^ ((m >> 1) & 3), rows every 64 bytes (8-row groups of 512 bytes).
 #pragma once
 #include <stdint.h>
 #include "../../include/cape_b200.h"
@@ -15,9 +16,13 @@ namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B (layout type 1), stride between 8-row groups 1024 B
+// wgmma shared-memory matrix descriptor: K-major, tile rows of ROW_BYTES = 128 (SWIZZLE_128B, layout type 1) or 64
+// (SWIZZLE_64B, layout type 2), stride between 8-row groups 8 * ROW_BYTES
+template <int ROW_BYTES = 128>
 __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
-  return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
+  static_assert(ROW_BYTES == 128 || ROW_BYTES == 64, "128- or 64-byte swizzle");
+  return (uint64_t)((smem_addr >> 4) & 0x3fffu) | (1ull << 16) | ((uint64_t)(8 * ROW_BYTES >> 4) << 32) |
+         ((ROW_BYTES == 128 ? 1ull : 2ull) << 62);
 }
 
 // byte offset of element (m, k) (k = 0..31) of a tile
@@ -97,16 +102,18 @@ __device__ __forceinline__ void split_store1(float v, char* hi_tile, char* lo_ti
   *reinterpret_cast<float*>(lo_tile + off) = v - h;
 }
 
-// acc += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo over one 32-deep chunk (four k-steps of 8), A = 64 rows of this warpgroup
-template <int N>
+// acc += A_hi.B_hi + A_lo.B_hi + A_hi.B_lo over the KS k-steps of 8 of one tile row (KS = 4: a 32-deep chunk with
+// the 128-byte swizzle; KS = 2: the 16-deep half of one with the 64-byte swizzle), A = 64 rows of this warpgroup
+template <int N, int KS = 4>
 __device__ __forceinline__ void mma3_chunk(float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi,
                                            uint32_t b_lo, int scale_first) {
+  constexpr int RB = 32 * KS;
 #pragma unroll
-  for (int ks = 0; ks < 4; ++ks) {
+  for (int ks = 0; ks < KS; ++ks) {
     const uint32_t adv = 32u * ks;
-    wg::mma_tf32<N>(d, make_desc(a_hi + adv), make_desc(b_hi + adv), ks == 0 ? scale_first : 1);
-    wg::mma_tf32<N>(d, make_desc(a_lo + adv), make_desc(b_hi + adv), 1);
-    wg::mma_tf32<N>(d, make_desc(a_hi + adv), make_desc(b_lo + adv), 1);
+    wg::mma_tf32<N>(d, make_desc<RB>(a_hi + adv), make_desc<RB>(b_hi + adv), ks == 0 ? scale_first : 1);
+    wg::mma_tf32<N>(d, make_desc<RB>(a_lo + adv), make_desc<RB>(b_hi + adv), 1);
+    wg::mma_tf32<N>(d, make_desc<RB>(a_hi + adv), make_desc<RB>(b_lo + adv), 1);
   }
 }
 

@@ -21,9 +21,13 @@
 // the column tiles and then the f tiles fastest, so the CTAs of one row split run together and read its A and G rows
 // from L2 rather than from HBM once per tile.
 //
-// Each row split is one accumulation chain (scale_d = 1 throughout), unlike the forward kernel's fresh accumulator per
-// chunk: the split plan bounds the chain's length.  Partial sums of the row splits go to the topology workspace and
-// are reduced deterministically (reduce_splits_kernel).
+// The tensor core's fp32 accumulation truncates, so a sum over a long chain of MMAs shrinks a little with every MMA;
+// the rows per split grow with the batch (the split plan keeps the number of CTAs fixed).  So every DW_FLUSH_CHUNKS
+// chunks (2048 rows, more than any split of the batch-64 step has) the consumers wait for their MMAs, add the
+// accumulators into the CTA's own output slice in fp32 (red.global: no round trip, no registers; the first flush
+// stores unless it accumulates into dW) and start the next chunk with scale_d = 0.  Each element has one owning
+// thread, so the order of the adds is fixed.  Partial sums of the row splits go to the topology workspace and are
+// reduced deterministically (reduce_splits_kernel).
 #include "common.cuh"
 #include "ellconv_params.cuh"
 #include "tc_common.cuh"
@@ -38,6 +42,7 @@ constexpr int DW_KCH = 32;                   // rows (K) per chunk
 constexpr int DW_A_TILE = 128 * 128;         // 128 f x 32 rows, hi or lo
 constexpr int DW_BAR_BYTES = 256;            // the ring's mbarriers
 constexpr int DW_SMEM_MAX = 227 * 1024;      // dynamic shared memory per CTA on sm_90
+constexpr int DW_FLUSH_CHUNKS = 64;          // chunks (2048 rows) per MMA chain, unless set by cape_set_tuning(11, .)
 
 struct DwTcParams {
   int rows_out, ncols, F, src_rows, src_stride;
@@ -49,6 +54,7 @@ struct DwTcParams {
   long long out_rs;
   int nsplit, accumulate;
   int ftiles, ctiles;
+  int flush_chunks;    // chunks per MMA chain: the consumers add their accumulators into `out` every flush_chunks
 };
 
 template <int BN>
@@ -71,7 +77,16 @@ struct DwCfg {
   static_assert(2 * STAGES * 8 <= DW_BAR_BYTES, "mbarrier area too small");
 };
 
-template <int BN>
+// *o += v in fp32 (round to nearest) by the L2, without a round trip to the issuing thread (red.global)
+__device__ __forceinline__ void red_add(float* o, float v) {
+  asm volatile("red.global.add.f32 [%0], %1;" ::"l"(__cvta_generic_to_global(o)), "f"(v) : "memory");
+}
+__device__ __forceinline__ void red_add2(float* o, float v0, float v1) {     // o 8-byte aligned
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(__cvta_generic_to_global(o)), "f"(v0), "f"(v1)
+               : "memory");
+}
+
+template <int BN, bool CHAINS>
 __global__ void __launch_bounds__(DwCfg<BN>::THREADS, 1) dw_wg_kernel(const __grid_constant__ DwTcParams p) {
   using Cfg = DwCfg<BN>;
   constexpr int S = Cfg::STAGES;
@@ -167,52 +182,103 @@ __global__ void __launch_bounds__(DwCfg<BN>::THREADS, 1) dw_wg_kernel(const __gr
   // =========================== consumers ===========================
   setmaxnreg_inc<Cfg::CONSUMER_REGS>();
   const int cw = wgi - Cfg::PRODUCERS, wt = tid & 127;
+  float* out = p.out + (p.nsplit > 1 ? (size_t)split * p.F * p.out_rs : 0);
+  const bool vec2 = (p.out_rs % 2 == 0) && ((reinterpret_cast<uintptr_t>(out) & 7u) == 0);
   float acc[NA];
 #pragma unroll
   for (int i = 0; i < NA; ++i) acc[i] = 0.f;
   fence_acc(acc);
-  for (long long kc = 0; kc < nchunks; ++kc) {
-    const int stage = (int)(kc % S);
-    mbar_wait(&full[stage], (uint32_t)((kc / S) & 1));
-    const uint32_t base = smem_u32(smem + (size_t)stage * Cfg::STAGE);
-    const uint32_t a_hi = base + (uint32_t)(cw * 64 * 128), a_lo = a_hi + DW_A_TILE;
-    const uint32_t g_hi = base + 2 * DW_A_TILE, g_lo = g_hi + Cfg::G_TILE;
-    wgmma_fence();
-    mma3_chunk<BN>(acc, a_hi, a_lo, g_hi, g_lo, 1);
-    wgmma_commit();
-    wgmma_wait<1>();                         // the previous chunk's MMAs have read their stage
-    if (kc > 0 && lane == 0) mbar_arrive(&empty[(int)((kc - 1) % S)]);
-  }
-  wgmma_wait<0>();
-  fence_acc(acc);
-
-  // =========================== epilogue: accumulators -> dW or the split's partial sums ===========================
-  float* out = p.out + (p.nsplit > 1 ? (size_t)split * p.F * p.out_rs : 0);
-  const bool vec2 = (p.out_rs % 2 == 0) && ((reinterpret_cast<uintptr_t>(out) & 7u) == 0);
+  if constexpr (!CHAINS) {
+    // ---- every split fits one chain: one pass, then the accumulators -> dW or the split's partial sums ----
+    for (long long kc = 0; kc < nchunks; ++kc) {
+      const int stage = (int)(kc % S);
+      mbar_wait(&full[stage], (uint32_t)((kc / S) & 1));
+      const uint32_t base = smem_u32(smem + (size_t)stage * Cfg::STAGE);
+      const uint32_t a_hi = base + (uint32_t)(cw * 64 * 128), a_lo = a_hi + DW_A_TILE;
+      const uint32_t g_hi = base + 2 * DW_A_TILE, g_lo = g_hi + Cfg::G_TILE;
+      wgmma_fence();
+      mma3_chunk<BN>(acc, a_hi, a_lo, g_hi, g_lo, 1);
+      wgmma_commit();
+      wgmma_wait<1>();                       // the previous chunk's MMAs have read their stage
+      if (kc > 0 && lane == 0) mbar_arrive(&empty[(int)((kc - 1) % S)]);
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
 #pragma unroll
-  for (int i = 0; i < NA; i += 2) {
-    const int f = ftile + cw * 64 + frag_row(wt, i);
-    const int c = col0 + frag_col(wt, i);
-    if (f >= p.F || c >= p.ncols) continue;
-    float* o = out + (size_t)f * p.out_rs + c;
-    if (p.nsplit == 1 && p.accumulate) {
-      o[0] += acc[i];
-      o[1] += acc[i + 1];
-    } else if (vec2) {
-      *reinterpret_cast<float2*>(o) = make_float2(acc[i], acc[i + 1]);
-    } else {
-      o[0] = acc[i];
-      o[1] = acc[i + 1];
+    for (int i = 0; i < NA; i += 2) {
+      const int f = ftile + cw * 64 + frag_row(wt, i);
+      const int c = col0 + frag_col(wt, i);
+      if (f >= p.F || c >= p.ncols) continue;
+      float* o = out + (size_t)f * p.out_rs + c;
+      if (p.nsplit == 1 && p.accumulate) {
+        o[0] += acc[i];
+        o[1] += acc[i + 1];
+      } else if (vec2) {
+        *reinterpret_cast<float2*>(o) = make_float2(acc[i], acc[i + 1]);
+      } else {
+        o[0] = acc[i];
+        o[1] = acc[i + 1];
+      }
+    }
+  } else {
+    // ---- chains of flush_chunks chunks: after each, the accumulators are stored into this CTA's slice of dW or of
+    // the split's partial sums (added into dW when accumulating) the first time and added in fp32 after that.  Each
+    // element has one owning thread, whose adds follow program order.
+    bool flushed = false;
+    auto flush = [&]() {
+      const bool add = flushed || (p.nsplit == 1 && p.accumulate);
+      // opaque to the compiler: the addresses are computed here, not kept live across the loop (no spare registers)
+      float* dst = out;
+      int t = wt;
+      asm volatile("" : "+l"(dst), "+r"(t));
+#pragma unroll
+      for (int i = 0; i < NA; i += 2) {
+        const int f = ftile + cw * 64 + frag_row(t, i);
+        const int c = col0 + frag_col(t, i);
+        if (f >= p.F || c >= p.ncols) continue;
+        float* o = dst + (size_t)f * p.out_rs + c;
+        if (add && vec2) {
+          red_add2(o, acc[i], acc[i + 1]);
+        } else if (add) {
+          red_add(o, acc[i]);
+          red_add(o + 1, acc[i + 1]);
+        } else if (vec2) {
+          *reinterpret_cast<float2*>(o) = make_float2(acc[i], acc[i + 1]);
+        } else {
+          o[0] = acc[i];
+          o[1] = acc[i + 1];
+        }
+      }
+      flushed = true;
+    };
+    for (long long k0 = 0; k0 < nchunks; k0 += p.flush_chunks) {
+      const long long k1 = min(nchunks, k0 + p.flush_chunks);
+      for (long long kc = k0; kc < k1; ++kc) {
+        const int stage = (int)(kc % S);
+        mbar_wait(&full[stage], (uint32_t)((kc / S) & 1));
+        const uint32_t base = smem_u32(smem + (size_t)stage * Cfg::STAGE);
+        const uint32_t a_hi = base + (uint32_t)(cw * 64 * 128), a_lo = a_hi + DW_A_TILE;
+        const uint32_t g_hi = base + 2 * DW_A_TILE, g_lo = g_hi + Cfg::G_TILE;
+        wgmma_fence();
+        mma3_chunk<BN>(acc, a_hi, a_lo, g_hi, g_lo, kc == k0 ? 0 : 1);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kc > 0 && lane == 0) mbar_arrive(&empty[(int)((kc - 1) % S)]);
+      }
+      wgmma_wait<0>();
+      fence_acc(acc);
+      flush();
     }
   }
 }
 
-template <int BN>
+template <int BN, bool CHAINS>
 int launch_dw(const DwTcParams& p, cudaStream_t st) {
   using Cfg = DwCfg<BN>;
   static bool configured = false;
   if (!configured) {
-    CAPE_CHECK_CUDA(cudaFuncSetAttribute(dw_wg_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    CAPE_CHECK_CUDA(cudaFuncSetAttribute(dw_wg_kernel<BN, CHAINS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         Cfg::SMEM_BYTES));
     configured = true;
   }
   const long long nblocks = (long long)p.ftiles * p.ctiles * p.nsplit;
@@ -220,10 +286,15 @@ int launch_dw(const DwTcParams& p, cudaStream_t st) {
     set_error("dw_wg_kernel: too many tiles");
     return -1;
   }
-  dw_wg_kernel<BN><<<(unsigned)nblocks, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(p);
+  dw_wg_kernel<BN, CHAINS><<<(unsigned)nblocks, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(p);
   CAPE_CHECK_CUDA(cudaGetLastError());
   count_launches(1);
   return 1;
+}
+
+template <int BN>
+int launch_dw(const DwTcParams& p, cudaStream_t st) {
+  return p.rows_per_split / DW_KCH > p.flush_chunks ? launch_dw<BN, true>(p, st) : launch_dw<BN, false>(p, st);
 }
 
 }  // namespace
@@ -253,6 +324,7 @@ int launch_ellconv_dw_tc(const cape_topology* t, const cape_dw_args* a, const Op
   rps = (rps + DW_KCH - 1) / DW_KCH * DW_KCH;
   nsplit = (p.total_rows + rps - 1) / rps;
   p.rows_per_split = rps; p.nsplit = (int)nsplit; p.accumulate = a->accumulate;
+  p.flush_chunks = g_tuning[11] > 0 ? g_tuning[11] : (g_tuning[11] < 0 ? INT_MAX : DW_FLUSH_CHUNKS);
   if (nsplit == 1) { p.out = a->dw; p.out_rs = a->dw_stride; }
   else { p.out = (float*)t->workspace; p.out_rs = a->ncols; }
   *nsplit_out = (int)nsplit;

@@ -83,7 +83,8 @@ int launch_ellconv_dw_tc(const cape_topology* t, const cape_dw_args* a, const Op
                          cudaStream_t st);
 
 // experiment knobs (cape_set_tuning): [7] = 1: thin-output layers on the generic kernels, [8] = 1: no tensor-core
-// plain-operand path, [10]: rows per cape_apply CTA, [16] = 1: scalar FC kernel, [17] = 1: fixed thin-dW CTA count
+// plain-operand path, [10]: rows per cape_apply CTA, [11]: chunks of 32 rows per MMA chain of dw_wg_kernel (0: 64,
+// < 0: one chain per row split), [16] = 1: scalar FC kernel, [17] = 1: fixed thin-dW CTA count
 extern int g_tuning[32];
 
 }  // namespace cape

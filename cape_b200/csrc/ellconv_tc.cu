@@ -628,7 +628,7 @@ int launch_gemm_tc(const cape_topology* t, const ConvParams& p, bool dual, cudaS
 }  // namespace cape
 
 extern "C" int cape_set_tuning(int key, int value) {
-  CAPE_REQUIRE(key == 7 || key == 8 || key == 10 || key == 16 || key == 17, "unknown tuning key");
+  CAPE_REQUIRE(key == 7 || key == 8 || key == 10 || key == 11 || key == 16 || key == 17, "unknown tuning key");
   const int prev = cape::g_tuning[key];
   cape::g_tuning[key] = value;
   return prev;

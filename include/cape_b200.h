@@ -161,7 +161,8 @@ int cape_apply(cape_topology* t, const cape_apply_args* a, void* stream);
 
 /* Experiment knobs (process-wide, all 0 by default = the shipped configuration).  They switch single
  * optimisations off for A/B measurements and fallback-path tests: [7]=1 thin-output layers on the generic kernels,
- * [8]=1 no tensor-core plain-operand conv path, [10]=rows per CTA of cape_apply (16..1024), [16]=1 scalar FC kernel,
+ * [8]=1 no tensor-core plain-operand conv path, [10]=rows per CTA of cape_apply (16..1024), [11]=chunks of 32 rows
+ * per MMA chain of the tensor-core weight gradient (0: 64, <0: one chain per row split), [16]=1 scalar FC kernel,
  * [17]=1 fixed CTA count of the thin weight gradient.  Returns the previous value, <0 for an unknown key. */
 int cape_set_tuning(int key, int value);
 

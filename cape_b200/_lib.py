@@ -102,6 +102,9 @@ SIGNATURES = {
     "cape_recon_losses_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                        C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
                                        C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cape_recon_losses_w": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                      C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p, C.c_double, C.c_void_p,
+                                      C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cape_bce_logits": (C.c_int, [C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cape_sumsq": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "cape_sgd_clip_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float,

@@ -1,6 +1,8 @@
 // Small fused kernels around the graph convolutions: re-parameterisation, losses, optimiser.
 // Reference: lib/models.py:193-196 (vae_sampling), :354-416 + lib/losses.py:9-25 (losses),
 // :419-474 (clip_by_global_norm + MomentumOptimizer).
+#include <cmath>
+
 #include "common.cuh"
 
 namespace cape {
@@ -71,6 +73,7 @@ struct ReconParams {
   float s_edge;   // 0.5 / (N*n_edges)   (every undirected edge is visited from both ends)
   float* dpred;
   float* losses;
+  const float* vweight;  // [rows] per-vertex weights of the reconstruction term (WEIGHTED instantiations only)
 };
 
 // the reconstruction term's value and gradient (before the lambda / count scale) of one coordinate's residual d
@@ -90,7 +93,10 @@ __device__ __forceinline__ float recon_term(float d, float delta, float* grad) {
   return a;
 }
 
-template <int KIND>
+// WEIGHTED: the reconstruction term of vertex v (its three coordinates' loss and gradient) is scaled by vweight[v], and
+// g_l1 / s_l1 divide by N * 3 * sum(vweight) instead of the coordinate count.  A template flag, so that the unweighted
+// instantiations compile to the code they had before the flag existed.
+template <int KIND, bool WEIGHTED>
 __global__ void __launch_bounds__(256) recon_kernel(const __grid_constant__ ReconParams p) {
   __shared__ float red[8];
   const long long total = (long long)p.N * p.rows;
@@ -105,9 +111,15 @@ __global__ void __launch_bounds__(256) recon_kernel(const __grid_constant__ Reco
     const float vx = recon_term<KIND>(dx, p.delta, &tx), vy = recon_term<KIND>(dy, p.delta, &ty),
                 vz = recon_term<KIND>(dz, p.delta, &tz);
     l1 = vx + vy + vz;
-    float gx = p.g_l1 * tx;
-    float gy = p.g_l1 * ty;
-    float gz = p.g_l1 * tz;
+    float g_l1 = p.g_l1;
+    if (WEIGHTED) {
+      const float m = __ldg(p.vweight + v);
+      l1 *= m;
+      g_l1 *= m;
+    }
+    float gx = g_l1 * tx;
+    float gy = g_l1 * ty;
+    float gz = g_l1 * tz;
     const int32_t* nb = p.nbr + (size_t)v * p.width;
     for (int j = 0; j < p.width; ++j) {
       const int u = __ldg(nb + j);
@@ -347,10 +359,11 @@ extern "C" int cape_vae_sample_bwd(const float* dz, int dz_stride, const float* 
   return 0;
 }
 
-extern "C" int cape_recon_losses_ex(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
-                                    int kind, float delta, float lambda_l1, float lambda_edge, int n_edges,
-                                    const float* mean, const float* logvar, int nz, float* dpred, float* losses,
-                                    void* stream) {
+// vweight: nullptr, or [rows] per-vertex weights with their sum vweight_sum (> 0)
+static int recon_losses(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows, int kind,
+                        float delta, float lambda_l1, float lambda_edge, int n_edges, const float* vweight,
+                        double vweight_sum, const float* mean, const float* logvar, int nz, float* dpred, float* losses,
+                        void* stream) {
   CAPE_REQUIRE(t && pred && gt && dpred && losses, "null pointer");
   CAPE_REQUIRE(kind == CAPE_RECON_L1 || kind == CAPE_RECON_L2 || kind == CAPE_RECON_HUBER, "unknown reconstruction loss");
   CAPE_REQUIRE(kind != CAPE_RECON_HUBER || delta > 0.f, "the Huber loss needs delta > 0");
@@ -360,17 +373,25 @@ extern "C" int cape_recon_losses_ex(cape_topology* t, int nbr_op, const float* p
   CAPE_REQUIRE(N > 0 && n_edges > 0, "empty problem");
   ReconParams p{};
   p.nbr = o.idx; p.width = o.width; p.pred = pred; p.gt = gt; p.N = N; p.rows = rows;
-  const double cnt = (double)N * rows * 3.0, ecnt = (double)N * n_edges;
+  // TF-1 Reduction.MEAN: the weighted sum over the sum of the weights broadcast to [N, rows, 3]
+  const double cnt = (double)N * (vweight ? vweight_sum : (double)rows) * 3.0, ecnt = (double)N * n_edges;
   p.g_l1 = (float)(lambda_l1 / cnt); p.g_edge = (float)(lambda_edge / ecnt);
   p.s_l1 = (float)(1.0 / cnt); p.s_edge = (float)(0.5 / ecnt);
   p.delta = delta;
   p.dpred = dpred; p.losses = losses;
+  p.vweight = vweight;
   const long long total = (long long)N * rows;
   cudaStream_t st = (cudaStream_t)stream;
   const unsigned blocks = (unsigned)((total + 255) / 256);
-  if (kind == CAPE_RECON_L2) recon_kernel<CAPE_RECON_L2><<<blocks, 256, 0, st>>>(p);
-  else if (kind == CAPE_RECON_HUBER) recon_kernel<CAPE_RECON_HUBER><<<blocks, 256, 0, st>>>(p);
-  else recon_kernel<CAPE_RECON_L1><<<blocks, 256, 0, st>>>(p);
+  if (vweight) {
+    if (kind == CAPE_RECON_L2) recon_kernel<CAPE_RECON_L2, true><<<blocks, 256, 0, st>>>(p);
+    else if (kind == CAPE_RECON_HUBER) recon_kernel<CAPE_RECON_HUBER, true><<<blocks, 256, 0, st>>>(p);
+    else recon_kernel<CAPE_RECON_L1, true><<<blocks, 256, 0, st>>>(p);
+  } else {
+    if (kind == CAPE_RECON_L2) recon_kernel<CAPE_RECON_L2, false><<<blocks, 256, 0, st>>>(p);
+    else if (kind == CAPE_RECON_HUBER) recon_kernel<CAPE_RECON_HUBER, false><<<blocks, 256, 0, st>>>(p);
+    else recon_kernel<CAPE_RECON_L1, false><<<blocks, 256, 0, st>>>(p);
+  }
   CAPE_CHECK_CUDA(cudaGetLastError());
   cape::count_launches(1);
   if (mean && logvar && nz > 0) {
@@ -379,6 +400,24 @@ extern "C" int cape_recon_losses_ex(cape_topology* t, int nbr_op, const float* p
   cape::count_launches(1);
   }
   return 0;
+}
+
+extern "C" int cape_recon_losses_ex(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
+                                    int kind, float delta, float lambda_l1, float lambda_edge, int n_edges,
+                                    const float* mean, const float* logvar, int nz, float* dpred, float* losses,
+                                    void* stream) {
+  return recon_losses(t, nbr_op, pred, gt, N, rows, kind, delta, lambda_l1, lambda_edge, n_edges, nullptr, 0.0, mean,
+                      logvar, nz, dpred, losses, stream);
+}
+
+extern "C" int cape_recon_losses_w(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
+                                   int kind, float delta, float lambda_l1, float lambda_edge, int n_edges,
+                                   const float* vweight, double vweight_sum, const float* mean, const float* logvar,
+                                   int nz, float* dpred, float* losses, void* stream) {
+  CAPE_REQUIRE(vweight, "null vertex weights");
+  CAPE_REQUIRE(vweight_sum > 0.0 && std::isfinite(vweight_sum), "the vertex weights must have a positive finite sum");
+  return recon_losses(t, nbr_op, pred, gt, N, rows, kind, delta, lambda_l1, lambda_edge, n_edges, vweight, vweight_sum,
+                      mean, logvar, nz, dpred, losses, stream);
 }
 
 extern "C" int cape_recon_losses(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,

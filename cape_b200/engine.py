@@ -367,6 +367,21 @@ def axpy(tp, y, x, a):
     check(tp.lib.cape_axpy(_ptr(y), _ptr(x), float(a), y.numel(), _stream()))
 
 
+def recon_losses(tp, nbr_op, pred, gt, N, rows, kind, lambda_recon, lambda_edge, n_edges, z_mean, z_logvar, nz, dpred,
+                 losses, mask=None, mask_sum=0.0):
+    """Reconstruction (of `kind`), edge and KL terms into losses[0..2], their lambda-weighted gradient added to dpred.
+    mask: None, or the device [rows] per-vertex weights of the reconstruction term (sum mask_sum) of the reference's
+    `--loss_mask binary` (lib/models.py:47-52,357-369) -> cape_recon_losses_w."""
+    head = (tp.h, nbr_op, _ptr(pred), _ptr(gt), N, rows, kind, HUBER_DELTA, float(lambda_recon), float(lambda_edge),
+            n_edges)
+    tail = (_ptr(z_mean), _ptr(z_logvar), nz, _ptr(dpred), _ptr(losses), _stream())
+    if mask is None:
+        check(tp.lib.cape_recon_losses_ex(*head, *tail))
+    else:
+        assert mask.numel() == rows and mask_sum > 0, "the loss mask needs one weight per vertex and a positive sum"
+        check(tp.lib.cape_recon_losses_w(*head, _ptr(_f32(mask)), float(mask_sum), *tail))
+
+
 def resample(tp, op, x, y, N, rows_out, rows_in, F, x_stride=None, y_stride=None, cond=None):
     check(tp.lib.cape_resample(tp.h, op, _ptr(x), F if x_stride is None else x_stride, _ptr(y),
                                F if y_stride is None else y_stride, N, rows_out, rows_in, F, _ptr(cond),

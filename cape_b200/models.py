@@ -34,8 +34,6 @@ class CAPE(object):
             raise NotImplementedError("kernels exist for filter='chebyshev5' and pool=unpool='poolwT' (the configuration "
                                       "of every shipped config)")
         E.brelu(activation)                  # b1leakyrelu, b1relu or b1tanh; anything else raises
-        if loss_mask == "binary":
-            raise NotImplementedError("loss_mask='binary' is broken in the reference too (lib/models.py:49-50)")
         self.Laplacian, self.Downsample_mtx, self.Upsample_mtx, self.p = L, D, U, p
         self.Laplacian_d, self.Downsample_mtx_d = L_d, D_d
         self.input_num_verts = L[0].shape[0]
@@ -58,7 +56,7 @@ class CAPE(object):
                         decay_steps=decay_steps if decay_steps else 1, momentum=momentum, lr_warmup=bool(lr_warmup),
                         optimizer=optimizer, regularization=regularization, lambda_recon=lambda_recon,
                         lambda_edge=lambda_edge, lambda_latent=lambda_latent, lambda_gan=lambda_gan, loss=loss,
-                        activation=activation,
+                        activation=activation, loss_mask=loss_mask if loss_mask == "binary" else None,
                         batch_size=int(batch_size), seed=seed)
         self.net = None
         self.rng = np.random.RandomState(seed)
@@ -316,7 +314,13 @@ class CAPE(object):
                 kind = E.recon_kind(self.cfg["loss"])               # the configured loss (models.py:357-369)
                 rest = (net.n_edges, E._ptr(net.z_mean), E._ptr(net.z_logvar), self.nz, E._ptr(net.d_xhat),
                       E._ptr(net.losses), E._stream())
-                if kind == E.RECON_L1:
+                if self.cfg["loss_mask"] == "binary":
+                    # the masked term (models.py:1073), the mask covering the whole zero-padded batch
+                    E.recon_losses(net.tp, net.nbr_op, net.x_hat, gt, N, net.p[0], kind, 0.0, 0.0, net.n_edges,
+                                   net.z_mean, net.z_logvar, self.nz, net.d_xhat, net.losses, mask=net.loss_mask,
+                                   mask_sum=net.loss_mask_sum)
+                    rc = 0
+                elif kind == E.RECON_L1:
                     rc = net.tp.lib.cape_recon_losses(net.tp.h, net.nbr_op, E._ptr(net.x_hat), E._ptr(gt), N, net.p[0],
                                                       0.0, 0.0, *rest)
                 else:

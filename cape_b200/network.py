@@ -824,6 +824,17 @@ class CapeNetwork:
             self.c_clo1, self.c_clo2 = dn("condition_clo_label/fc1"), None
         self.nbr_op = tp.add_operator(_adjacency(L[0]))
         self.n_edges = int(_adjacency(L[0]).nnz // 2)
+        # `--loss_mask binary` (models.py:47-52): per-vertex weights of the reconstruction term; any other value: none.
+        # Indexed by the reference's vertex numbering, which x_hat keeps whatever `reorder` says (dec/outputs has no
+        # order_out).
+        self.loss_mask, self.loss_mask_sum = None, 0.0
+        if c.get("loss_mask") == "binary":
+            m = topo.loss_mask_binary()
+            if m.shape[0] != self.p[0]:
+                raise ValueError("loss_mask='binary' weights the %d SMPL vertices; this mesh has %d"
+                                 % (m.shape[0], self.p[0]))
+            self.loss_mask = torch.from_numpy(m).to(dev)
+            self.loss_mask_sum = float(m.astype(np.float64).sum())
         self.arena.build(dev)
         self.scratch = torch.empty(self._scratch_need, device=dev)
 
@@ -1232,10 +1243,9 @@ class CapeNetwork:
         # gradient buffers the discriminator's weight gradients are still reading on the side stream: join first)
         self.join_dw()
         self.disc_bwd(N, 2 * N, self.d_logits_g, want_dw=False, dx=self.d_xhat, dycat=self.d_ycat, cs_slot=1)
-        _lib.check(lib.cape_recon_losses_ex(tp.h, self.nbr_op, E._ptr(self.x_hat), E._ptr(self.in_x), N, self.p[0],
-                                            self.recon_kind, E.HUBER_DELTA, float(c["lambda_recon"]),
-                                            float(c["lambda_edge"]), self.n_edges, E._ptr(self.z_mean),
-                                            E._ptr(self.z_logvar), self.nz, E._ptr(self.d_xhat), E._ptr(L), st()))
+        E.recon_losses(tp, self.nbr_op, self.x_hat, self.in_x, N, self.p[0], self.recon_kind, c["lambda_recon"],
+                       c["lambda_edge"], self.n_edges, self.z_mean, self.z_logvar, self.nz, self.d_xhat, L,
+                       mask=self.loss_mask, mask_sum=self.loss_mask_sum)
         self.decoder_bwd()
         self._fc_reg(("generator/decoder/fc1",))
         if not self.side_glue:

@@ -16,6 +16,7 @@ of A[0], checked against the reference file), the per-vertex normalisation stati
 poses (demos.py:349-357).
 
     python -m cape_b200.pack_topology --reference /path/to/CAPE        (default: $CAPE_REFERENCE)
+    python -m cape_b200.pack_topology --loss-mask                      (tests/golden/loss_mask_binary.npz only)
 """
 import argparse
 import os
@@ -82,13 +83,29 @@ def pack(REF, OUT=OUT):
     return OUT
 
 
+def pack_loss_mask(REF, OUT=OUT):
+    """data/loss_mask_binary.npy (the per-vertex weights of `--loss_mask binary`, lib/models.py:47-52) ->
+    <OUT>/loss_mask_binary.npz, float32 [6890].  The reference ships the mask 1-D, one weight per vertex."""
+    m = np.load(os.path.join(REF, "data", "loss_mask_binary.npy"))
+    if m.ndim != 1:
+        raise ValueError("expected one weight per vertex, got shape %s" % (m.shape,))
+    os.makedirs(OUT, exist_ok=True)
+    path = os.path.join(OUT, "loss_mask_binary.npz")
+    np.savez_compressed(path, loss_mask_binary=m.astype(np.float32))
+    return path
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--reference", default=default_reference(), help="checkout of qianlim/CAPE")
-    ap.add_argument("--out", default=OUT, help="directory of the two .npz files")
+    ap.add_argument("--out", default=OUT, help="directory of the .npz files")
+    ap.add_argument("--loss-mask", action="store_true", help="write only loss_mask_binary.npz")
     a = ap.parse_args(argv)
     if not a.reference:
         ap.error("no reference checkout found: pass --reference or set CAPE_REFERENCE")
+    if a.loss_mask:
+        print("wrote", pack_loss_mask(a.reference, a.out))
+        return 0
     out = pack(a.reference, a.out)
     print("wrote smpl_topology_{%s}.npz to %s" % (",".join(PARTS), os.path.abspath(out)))
 

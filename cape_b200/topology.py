@@ -17,6 +17,7 @@ import scipy.sparse as sp
 
 _DATA = [os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests", "golden",
                       "smpl_topology_%s.npz" % part) for part in ("for_demo", "ds2", "assets")]
+_LOSS_MASK = os.path.join(os.path.dirname(_DATA[0]), "loss_mask_binary.npz")
 _cache = {}
 
 
@@ -88,6 +89,15 @@ def trainset_stats():
 
 def clothing_verts_idx():
     return _npz()["clothing_verts_idx"]
+
+
+def loss_mask_binary():
+    """[6890] float32 per-vertex weights of `--loss_mask binary` (the reference's data/loss_mask_binary.npy, read at
+    lib/models.py:47-50): 1.0 on clothing-related vertices, 0.1 elsewhere."""
+    if "loss_mask" not in _cache:
+        with np.load(_LOSS_MASK) as f:
+            _cache["loss_mask"] = f["loss_mask_binary"]
+    return _cache["loss_mask"]
 
 
 def template_mesh():

@@ -305,6 +305,17 @@ enum { CAPE_RECON_L1 = 0, CAPE_RECON_L2 = 1, CAPE_RECON_HUBER = 2 };
 int cape_recon_losses_ex(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
                          int kind, float delta, float lambda_recon, float lambda_edge, int n_edges,
                          const float* mean, const float* logvar, int nz, float* dpred, float* losses, void* stream);
+/* cape_recon_losses_ex with per-vertex weights on the reconstruction term: the reference's `--loss_mask binary`
+ * (models.py:47-52 builds weights [N, rows, 1] from one per-vertex mask, :357-369 hands them to every loss kind).
+ * vweight: device [rows], m[v]; vweight_sum: sum_v m[v] (> 0).  TF-1 Reduction.MEAN divides the weighted sum by the
+ * sum of the weights broadcast to [N, rows, 3]:
+ *   losses[0] = sum_{n,v,c} m[v] l(d) / (3 N vweight_sum),  dpred += lambda_recon m[v] l'(d) / (3 N vweight_sum)
+ * with l, l' those of `kind`.  The edge and KL terms are cape_recon_losses_ex's, unweighted.  An all-ones vweight
+ * (sum rows) gives bit-identical results to cape_recon_losses_ex. */
+int cape_recon_losses_w(cape_topology* t, int nbr_op, const float* pred, const float* gt, int N, int rows,
+                        int kind, float delta, float lambda_recon, float lambda_edge, int n_edges,
+                        const float* vweight, double vweight_sum,
+                        const float* mean, const float* logvar, int nz, float* dpred, float* losses, void* stream);
 /* Sigmoid cross-entropy with a constant label (tf.nn.sigmoid_cross_entropy_with_logits, models.py:387-389):
  * loss[0] += mean(bce(logits, label)); dlogits = scale * d mean(bce)/dlogits  */
 int cape_bce_logits(const float* logits, int64_t n, float label, float scale, float* dlogits, float* loss,

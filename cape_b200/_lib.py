@@ -111,6 +111,10 @@ SIGNATURES = {
                                        C.c_void_p, C.c_float, C.c_void_p]),
     "cape_adam_clip_update": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_float,
                                         C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_void_p]),
+    "cape_histogram": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p]),
+    "cape_loss_ema": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
+                                C.c_float, C.c_void_p, C.c_void_p]),
     "cape_gn_relu_fwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cape_gn_relu_bwd": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,

@@ -47,7 +47,8 @@ def main(argv=None, project_dir=None):
     params = model_params(args, n_train=len(bodydata.vertices_train) if args.mode == "train" else None)
     params["p"] = p
     print("Building model graph...")
-    model = CAPE(L=L, D=D, U=U, L_d=L_ds2, D_d=D_ds2, **params)
+    # training writes TensorBoard summaries to summaries/<name>, relative to the working directory like checkpoints/
+    model = CAPE(L=L, D=D, U=U, L_d=L_ds2, D_d=D_ds2, summary_dir="summaries" if args.mode == "train" else None, **params)
     if args.mode == "train":
         model.build_graph(model.input_num_verts, model.nn_input_channel, phase="train")
         return model.fit(bodydata)

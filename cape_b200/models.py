@@ -15,6 +15,7 @@ import torch
 
 from . import _lib
 from . import engine as E
+from . import summary as S
 from .network import CapeNetwork
 from .params import DEFAULTS
 
@@ -27,7 +28,7 @@ class CAPE(object):
                  lr=0.008, decay_rate=0.99, optimizer="sgd", decay_steps=None, momentum=0.9, cond_dim=0, nz_cond=0,
                  regularization=0, batch_size=32, seed=123, lambda_recon=1.0, lambda_edge=0.0, lambda_latent=1e-3,
                  restart=False, name="", loss_mask=None, device=0, ref_compat=True, checkpoint_dir="checkpoints",
-                 device_dataset=True, **unused):
+                 device_dataset=True, summary_dir=None, **unused):
         # name-based operator seam of base_model (lib/models.py:58-62): kernels exist for chebyshev5 / poolwT and the
         # one-bias-per-filter activations
         if (filter, pool, unpool) != ("chebyshev5", "poolwT", "poolwT"):
@@ -45,6 +46,8 @@ class CAPE(object):
         self.lambda_l1, self.lambda_edge, self.lambda_latent = lambda_recon, lambda_edge, lambda_latent
         self.device_index, self.ref_compat, self.checkpoint_dir = device, ref_compat, checkpoint_dir
         self.device_dataset = bool(device_dataset)
+        # TensorBoard summaries of `fit` under <summary_dir>/<name> (the reference's `summaries` folder); None: none
+        self.summary_dir = summary_dir
         rd = reduce_dim if not isinstance(reduce_dim, bool) else (64 if reduce_dim else 0)
         if rd < 0:
             raise ValueError("reduce dim must be greater than 0!")           # lib/models.py:259
@@ -235,6 +238,7 @@ class CAPE(object):
         dev = None
         if self.device_dataset:
             dev = DeviceDataset(train_data, train_cond, train_cond2, net.device)
+        writer = self._open_summaries() if (self.summary_dir is not None and rank == 0) else None
         losses = []
         indices_g, indices_d = collections.deque(), collections.deque()
         for step in range(start_step, start_step + num_steps):
@@ -258,12 +262,55 @@ class CAPE(object):
                 net.train_step(step=self.global_step, allreduce=allreduce)
                 self.global_step += 2
             if (step % num_steps_epoch == 0 or step == num_steps) and rank == 0:
+                summary = self._summary_values() if writer is not None else None
                 string, recon, latent, edge = self.evaluate(*val)
                 losses.append(recon)
                 print("step {} / {}: validation {}  time: {:.0f}s".format(step, num_steps, string, time.time() - t_start))
+                if writer is not None:
+                    scalars, histograms = summary
+                    writer.add(step, scalars + [(S.VALIDATION_TAG, recon)], histograms)
                 self.save(step)
+        if writer is not None:
+            writer.close()
         t_step = (time.time() - t_start) / max(num_steps, 1)
         return losses, t_step
+
+    # ---- TensorBoard summaries (lib/models.py:868,919-922) -------------------------------------------------------------
+    def _open_summaries(self):
+        """A new event file in <summary_dir>/<name>.  At restart the reference deletes that folder (models.py:861); here
+        only the event files directly in it go.  The moving averages start at 0 with every `fit`."""
+        path = self._get_path(self.summary_dir)
+        if self.restart is True:
+            S.remove_event_files(path)
+        self.net.track_loss_average()
+        # the summary pass's own noise: training draws exactly what it draws without summaries
+        self._summary_rng = np.random.RandomState(self.cfg["seed"])
+        return S.EventWriter(path)
+
+    def _summary_values(self):
+        """sess.run(op_summary) on the loop step's batch (models.py:919): one more forward pass of both players at the
+        updated weights with fresh noise, no training op.  Returns ([(tag, value)], [(tag, HistogramProto bytes)])."""
+        net, c = self.net, self.cfg
+        eps = self._summary_rng.normal(size=(self.batch_size, self.nz)).astype(np.float32)
+        net.in_eps.copy_(torch.from_numpy(eps))
+        net.enqueue_loss_forward()
+        net.enqueue_fc_sumsq()
+        hist = net.weight_histograms()
+        v = net.losses.cpu().numpy()
+        avg = net.loss_avg.cpu().numpy()
+        f32 = np.float32
+        r = f32(c["regularization"])
+        reg_g = r * (r * (net.fc_sumsq.cpu().numpy()[0] * f32(0.5)))       # r * sum_W r * l2_loss(W), as cape_loss_ema
+        lr_g, lr_d = net.lr_now(self.global_step)
+        scalars = list(zip(S.SCALAR_TAGS, [v[0], v[2], reg_g, 0.0, v[3], v[4] + v[5], avg[0], avg[1], lr_g, lr_d]))
+        limits = S.bucket_limits()
+        histograms = []
+        for name in net.histogram_names():
+            stats, nonfinite, counts = hist[name]
+            if nonfinite:
+                raise ValueError("Nan in summary histogram for: %s" % name)
+            histograms.append((name, S.encode_histogram(stats, counts, limits)))
+        return scalars, histograms
 
     # ---- inference entry points (lib/models.py:931-1174) --------------------------------------------------------
     def encode(self, data=None, cond=None, cond2=None):

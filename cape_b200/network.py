@@ -16,6 +16,7 @@ import torch
 
 from . import _lib
 from . import engine as E
+from . import summary as S
 from . import topology as topo
 from .engine import (ACT_LEAKY, ACT_NONE, EPI_AFFINE, EPI_DUALMASK, EPI_LINEAR, EPI_SLOPE, ConvSite, Topology,
                      act_bwd, axpy, cheb_call, cheb_dw, colsum, gemm)
@@ -898,6 +899,7 @@ class CapeNetwork:
         self.losses = z(8)       # recon, edge, kl, gan_g, gan_d_real, gan_d_fake
         self.sumsq = z(2)
         self.lr = z(2)
+        self.loss_avg = None                # moving averages of loss_g / loss_d: track_loss_average()
         self._lr_host = torch.zeros(256, 2).pin_memory()   # ring: the async H2D of step k must not see step k+1's value
         self._lr_slot = 0
         self.step_count = 0
@@ -1210,16 +1212,11 @@ class CapeNetwork:
             k = math.floor(step / ds)
         return lr_g * c["decay_rate"] ** k, lr_d * c["decay_rate"] ** k
 
-    def enqueue_fwd_bwd(self):
-        """Forward + backward of both players for the staged batch; pure device work (CUDA-graph capturable)."""
-        N, c, tp = self.N, self.cfg, self.tp
-        lam_gan = float(c["lambda_gan"])
-        self.arena.zero()
-        self.losses.zero_()
-        self.d_ycat.zero_()
-        if not (self.affine or self.plain_dec):
-            self.PG.grad.zero_()          # group-norm gamma/beta gradients are accumulated by their kernels
-        # forward: both condition batches at once, generator, discriminator on [real ; fake]
+    def _forward_gan(self):
+        """The forward half up to the GAN losses: both condition batches at once, generator, discriminator on
+        [real ; fake], the three BCE terms into losses[3:6] (and their logit gradients)."""
+        N, tp = self.N, self.tp
+        lam_gan = float(self.cfg["lambda_gan"])
         self.cond_fwd(0, 2 * N)
         self.encoder_fwd()
         self.sample_fwd()
@@ -1236,6 +1233,31 @@ class CapeNetwork:
                                        E._ptr(L[4:]), st()))
         _lib.check(lib.cape_bce_logits(E._ptr(self.logits[N:]), nlog, 0.1, lam_gan, E._ptr(self.d_logits[N:]),
                                        E._ptr(L[5:]), st()))
+
+    def _recon_losses(self):
+        """Reconstruction, edge and KL terms into losses[0:3]; their gradient is added to d_xhat."""
+        c = self.cfg
+        E.recon_losses(self.tp, self.nbr_op, self.x_hat, self.in_x, self.N, self.p[0], self.recon_kind, c["lambda_recon"],
+                       c["lambda_edge"], self.n_edges, self.z_mean, self.z_logvar, self.nz, self.d_xhat, self.losses,
+                       mask=self.loss_mask, mask_sum=self.loss_mask_sum)
+
+    def enqueue_loss_forward(self):
+        """The training step's forward half alone, on the staged batch and the current weights: `losses` holds every
+        loss term afterwards.  No weight gradient is taken; d_xhat and the logit gradients, which the next step
+        rewrites before reading, are left dirty."""
+        self.losses.zero_()
+        self._forward_gan()
+        self._recon_losses()
+
+    def enqueue_fwd_bwd(self):
+        """Forward + backward of both players for the staged batch; pure device work (CUDA-graph capturable)."""
+        N, c, tp = self.N, self.cfg, self.tp
+        self.arena.zero()
+        self.losses.zero_()
+        self.d_ycat.zero_()
+        if not (self.affine or self.plain_dec):
+            self.PG.grad.zero_()          # group-norm gamma/beta gradients are accumulated by their kernels
+        self._forward_gan()
         # discriminator-loss path: weight gradients from both halves
         if not self.ref_compat:
             self.disc_bwd(0, 2 * N, self.d_logits, want_dw=True)
@@ -1243,9 +1265,7 @@ class CapeNetwork:
         # gradient buffers the discriminator's weight gradients are still reading on the side stream: join first)
         self.join_dw()
         self.disc_bwd(N, 2 * N, self.d_logits_g, want_dw=False, dx=self.d_xhat, dycat=self.d_ycat, cs_slot=1)
-        E.recon_losses(tp, self.nbr_op, self.x_hat, self.in_x, N, self.p[0], self.recon_kind, c["lambda_recon"],
-                       c["lambda_edge"], self.n_edges, self.z_mean, self.z_logvar, self.nz, self.d_xhat, L,
-                       mask=self.loss_mask, mask_sum=self.loss_mask_sum)
+        self._recon_losses()
         self.decoder_bwd()
         self._fc_reg(("generator/decoder/fc1",))
         if not self.side_glue:
@@ -1388,6 +1408,8 @@ class CapeNetwork:
             self.enqueue_fwd_bwd()
         if allreduce is not None and self.dp is None:
             allreduce(self.PG.grad, self.PD.grad)
+        if update and self.loss_avg is not None:
+            self.enqueue_loss_average()
         if update:
             if use_graph:
                 self.graph_up.replay()
@@ -1396,6 +1418,58 @@ class CapeNetwork:
             self.step_count = step + 1
             self.adam_t += 1
         return self.losses
+
+    # ---- TensorBoard summaries (lib/models.py:393-414, 217-227) ------------------------------------------------------
+    def track_loss_average(self):
+        """From now on every optimiser application also advances the moving averages of loss_g / loss_d
+        (`loss_avg`, starting at 0), outside the captured graphs."""
+        if self.loss_avg is None:
+            self.loss_avg = torch.zeros(2, device=self.device)
+            self.fc_sumsq = torch.zeros(1, device=self.device)
+
+    def enqueue_fc_sumsq(self):
+        """fc_sumsq = sum of W^2 over the generator's regularised dense kernels, at the current weights."""
+        self.fc_sumsq.zero_()
+        for n in S.FC_REGULARISED:
+            W = self._w(n)
+            _lib.check(self.tp.lib.cape_sumsq(E._ptr(W), W.numel(), E._ptr(self.fc_sumsq), E._stream()))
+
+    def enqueue_loss_average(self):
+        """Advance the moving averages with the losses of the application that just ran (its weights not yet updated)."""
+        c = self.cfg
+        self.enqueue_fc_sumsq()
+        _lib.check(self.tp.lib.cape_loss_ema(E._ptr(self.losses), E._ptr(self.fc_sumsq), float(c["lambda_gan"]),
+                                             float(c["lambda_recon"]), float(c["lambda_edge"]),
+                                             float(c["lambda_latent"]), float(c["regularization"]),
+                                             S.LOSS_AVERAGE_DECAY, E._ptr(self.loss_avg), E._stream()))
+
+    def histogram_names(self):
+        return S.histogram_names(self.specs)
+
+    def weight_histograms(self):
+        """{variable name: (stats, nonfinite, counts)} of every histogrammed variable at the current weights:
+        stats = float64 [min, max, num, sum, sum_squares], counts int64 over summary.bucket_limits().  One
+        cape_histogram launch and one device-to-host copy."""
+        if not hasattr(self, "_hist"):
+            names = self.histogram_names()
+            segs = torch.tensor([[self._w(n).data_ptr(), self._w(n).numel()] for n in names], dtype=torch.int64)
+            limits = S.bucket_limits()
+            nseg, nlim = len(names), len(limits)
+            # one 8-byte-word buffer: stats [nseg, 5] (double), nonfinite [nseg], counts [nseg, nlim]
+            self._hist = dict(names=names, segs=segs.to(self.device), nlim=nlim,
+                              limits=torch.from_numpy(limits).to(self.device),
+                              out=torch.zeros(nseg * (6 + nlim), dtype=torch.int64, device=self.device))
+        h = self._hist
+        names, nlim, out = h["names"], h["nlim"], h["out"]
+        nseg = len(names)
+        _lib.check(self.tp.lib.cape_histogram(self.tp.h, E._ptr(h["segs"]), nseg, E._ptr(h["limits"]), nlim,
+                                              E._ptr(out), E._ptr(out[5 * nseg:]), E._ptr(out[6 * nseg:]),
+                                              E._stream()))
+        host = out.cpu().numpy()
+        stats = host[:5 * nseg].view(np.float64).reshape(nseg, 5)
+        nonfinite = host[5 * nseg:6 * nseg]
+        counts = host[6 * nseg:].reshape(nseg, nlim)
+        return {n: (stats[i], int(nonfinite[i]), counts[i]) for i, n in enumerate(names)}
 
     def loss_dict(self):
         """Host copy of the last step's loss terms (synchronises)."""

@@ -338,6 +338,33 @@ int cape_sgd_clip_update(float* w, const float* g, float* mom, int64_t n, const 
 int cape_adam_clip_update(float* w, const float* g, float* m, float* v, int64_t n, const float* sumsq, float clip_norm,
                           const float* lr_t_dev, float beta1, float beta2, float eps, void* stream);
 
+/* ---- TensorBoard summaries (CAPE.fit's FileWriter, lib/models.py:868,919-922) --------------------------------------
+ * cape_histogram replaces tf.summary.histogram (lib/models.py:219,226) as TF-1.13's HistogramSummary evaluates it,
+ * for many variables in one launch.  segs: device array of nseg segments (views of the parameters); limits: device
+ * [nlim] ascending bucket limits, the last one DBL_MAX.  Every value is compared in double; for segment s:
+ *   counts[s, b] = #{x finite : b = upper_bound(limits, x)}  (limits[b-1] <= x < limits[b])
+ *   stats[s, :] = min, max, num, sum, sum of squares of its finite values, in double (min = DBL_MAX, max = -DBL_MAX
+ *   when there is none); nonfinite[s] = number of NaN / Inf values (TF refuses those: "Nan in summary histogram").
+ * The double sums are reduced in a fixed order: two calls give identical bits.  Uses the topology workspace
+ * (1796 bytes per segment); calls on one handle must be ordered. */
+typedef struct {
+  const float* p;
+  int64_t n;
+} cape_hist_segment;
+int cape_histogram(cape_topology* t, const cape_hist_segment* segs, int nseg, const double* limits, int nlim,
+                   double* stats, int64_t* nonfinite, int64_t* counts, void* stream);
+/* The moving averages of the loss totals (tf.train.ExponentialMovingAverage(decay).apply([loss_g, loss_d]),
+ * lib/models.py:393-414, zero_debias off), advanced once per optimiser application.  losses: the step's loss buffer
+ * (recon, edge, kl, gan_g, gan_d_real, gan_d_fake); fc_sumsq: sum of W^2 over the generator's regularised dense
+ * kernels (cape_sumsq).  In fp32, each operation rounded on its own, left to right as the reference writes them:
+ *   reg_g  = r * (r * (fc_sumsq * 0.5))                                    (r * sum_W r * l2_loss(W))
+ *   loss_g = gan_g * l_gan + recon * l_recon + 0 + edge * l_edge + kl * l_latent + reg_g
+ *   loss_d = (gan_d_real + gan_d_fake) * l_gan + 0
+ *   shadow[i] -= (shadow[i] - loss_i) * (1 - decay)
+ * One thread; no host synchronisation. */
+int cape_loss_ema(const float* losses, const float* fc_sumsq, float lambda_gan, float lambda_recon, float lambda_edge,
+                  float lambda_latent, float regularization, float decay, float* shadow, void* stream);
+
 /* ---- group norm (CAPE.gn, lib/models.py:681-712) + ReLU, for the non-affine decoder blocks ------------
  * x: [N, rows, C], G groups of C/G contiguous channels; stats over (C/G x rows) per (n, g), biased variance,
  * y = relu(gamma*(x-mean)*rstd + beta).  stats: [N, G, 2] = (mean, rstd), saved for the backward pass.
